@@ -229,6 +229,8 @@ typedef struct b200pg_summary {
   float setup_ms;              /* host time before the first kernel: flatten / adjacency / uploads of what changed */
   float wall_ms;               /* host wall time of the whole call                     */
   int32_t uploaded_edges;      /* constraints copied to the device by this call (the ones added since the last solve) */
+  int32_t linear_solver;       /* PCG kernel the plan chose: 0 global block-Jacobi, 1 shared-memory block-Jacobi,
+                                * 3 two-level with 3 coarse modes, 6 two-level with 6 coarse modes; -1 no linear solve planned */
 } b200pg_summary;
 
 typedef struct b200pg b200pg;

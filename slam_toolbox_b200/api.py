@@ -71,7 +71,7 @@ class PgSummary(C.Structure):
     _fields_ = [("iterations", C.c_int32), ("successful_steps", C.c_int32), ("pcg_iterations", C.c_int32),
                 ("termination", C.c_int32), ("usable", C.c_int32), ("initial_cost", C.c_double), ("final_cost", C.c_double),
                 ("solve_ms", C.c_float), ("kernel_launches", C.c_int64),
-                ("setup_ms", C.c_float), ("wall_ms", C.c_float), ("uploaded_edges", C.c_int32)]
+                ("setup_ms", C.c_float), ("wall_ms", C.c_float), ("uploaded_edges", C.c_int32), ("linear_solver", C.c_int32)]
 
 
 def library_path() -> str:

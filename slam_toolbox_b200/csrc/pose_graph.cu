@@ -1349,6 +1349,7 @@ static int solve(b200pg * h, b200pg_summary * sum)
   const b200pg_opts & o = h->o;
   b200pg_summary S{};
   S.usable = 1;
+  S.linear_solver = -1;
   const int N = (int)h->node_ids.size();
   if (N == 0) {   // "Ceres was called when there are no nodes" (ceres_solver.cpp:219-225)
     set_last_error("b200pg_solve: no nodes");
@@ -1522,6 +1523,7 @@ static int solve(b200pg * h, b200pg_summary * sum)
       c2.grc = h->d_grc.p; c2.e1 = h->d_e1.p; c2.e2 = h->d_e2.p; c2.bar = h->d_bar.p; c2.gjflag = h->d_bar.p + 1;
     }
   }
+  S.linear_solver = L.use_2lvl ? L.cm2 : L.use_smem ? 1 : 0;
   S.setup_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_enter).count();
   B200_CUDA(cudaEventRecord(h->ev0, st));
   // ---- iteration 0: evaluate, Jacobi scaling from the unscaled Jacobian ----

@@ -320,3 +320,194 @@ def make_pose_graph(seed: int, n_nodes: int = 10000, n_edges: int = 40000, latti
         init[i, 2] = wrap(init[i - 1, 2] + z[i - 1, 2])
     ids = np.arange(n_nodes, dtype=np.int32)
     return dict(ids=ids, init=init, truth=truth, edge_a=ea, edge_b=eb, z=z, cov=cov)
+
+
+def _pose_rel(pa, pb):
+    """pb in the frame of pa, rows (x, y, theta) -> (dx, dy, wrap(dtheta))."""
+    c, s = np.cos(pa[:, 2]), np.sin(pa[:, 2])
+    dx, dy = pb[:, 0] - pa[:, 0], pb[:, 1] - pa[:, 1]
+    return np.column_stack([c * dx + s * dy, -s * dx + c * dy, wrap(pb[:, 2] - pa[:, 2])])
+
+
+def _lattice_walk(rng: np.random.Generator, n: int, lattice: int, start) -> np.ndarray:
+    """Random walk of n lattice sites (1 m steps, 90 deg turns) inside [0, lattice)^2; returns (n, 3) cells + heading index."""
+    dirs = np.array([[1, 0], [0, 1], [-1, 0], [0, -1]])
+    out = np.zeros((n, 3), dtype=np.int64)
+    out[0, :2] = start
+    for i in range(1, n):
+        h = out[i - 1, 2]
+        r = rng.random()
+        h = (h + 1) % 4 if r < 0.25 else (h + 3) % 4 if r < 0.5 else h
+        nxt = out[i - 1, :2] + dirs[h]
+        while not (0 <= nxt[0] < lattice and 0 <= nxt[1] < lattice):
+            h = (h + 1) % 4
+            nxt = out[i - 1, :2] + dirs[h]
+        out[i, :2], out[i, 2] = nxt, h
+    return out
+
+
+def _base_covariance(rng: np.random.Generator, model: str, sigma_xy: float, sigma_th: float) -> np.ndarray:
+    """Edge covariance before the LinkInfo rotation.  iso: diag(sxy^2, sxy^2, sth^2).  karto: an anisotropic xy block
+    R(phi) diag(s1^2, s2^2) R(phi)^T with s1 / s2 in [1, 10] (a corridor) and a separate theta variance.  full: the karto
+    xy block with x-theta and y-theta correlations, a general SPD 3x3."""
+    if model == "iso":
+        return np.diag([sigma_xy ** 2, sigma_xy ** 2, sigma_th ** 2])
+    ratio = rng.uniform(1.0, 10.0)
+    s1, s2 = sigma_xy * math.sqrt(ratio), sigma_xy / math.sqrt(ratio)
+    phi = rng.uniform(-math.pi, math.pi)
+    c, s = math.cos(phi), math.sin(phi)
+    R = np.array([[c, -s], [s, c]])
+    cov = np.zeros((3, 3))
+    cov[:2, :2] = R @ np.diag([s1 * s1, s2 * s2]) @ R.T
+    cov[2, 2] = (sigma_th * rng.uniform(0.5, 2.0)) ** 2
+    if model == "full":
+        # correlation of theta with a random xy direction, |rho| <= 0.7: the Schur complement stays positive definite
+        rho = rng.uniform(-0.7, 0.7)
+        u = rng.normal(size=2)
+        u /= np.linalg.norm(u)
+        sd = np.sqrt(np.diag(cov[:2, :2]))
+        w = rho * math.sqrt(cov[2, 2]) * (cov[:2, :2] @ u) / math.sqrt(u @ cov[:2, :2] @ u)
+        cov[:2, 2] = cov[2, :2] = w
+        assert np.all(np.abs(w) < sd * math.sqrt(cov[2, 2]))
+    elif model != "karto":
+        raise ValueError(f"unknown covariance model {model!r}")
+    return cov
+
+
+def _rot_z(t: float) -> np.ndarray:
+    c, s = math.cos(t), math.sin(t)
+    return np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]])
+
+
+def make_pose_graph_family(seed: int, n_nodes: int = 2000, n_loops: int = 4000, *, cov_model: str = "iso",
+                           sigma_xy: float = 0.03, sigma_th: float = 0.01, reversed_frac: float = 0.0,
+                           duplicate_frac: float = 0.0, order: str = "chain", ids: str = "dense",
+                           world_rotation: float = 0.0, world_translation=(0.0, 0.0), isolated_runs=(),
+                           detached_nodes: int = 0, hub_degree: int = 0, lattice: int = 60, min_gap: int = 20,
+                           heading_jitter: float = 0.05) -> dict:
+    """SE(2) pose graphs of the shapes a mapper produces and make_pose_graph does not (it stays as it is: bench.py's cfg4).
+
+    A lattice random walk of n_nodes poses (headings jittered off the lattice directions) with odometry and up to
+    n_loops loop edges between poses on the same / adjacent site, plus:
+      cov_model        'iso' | 'karto' | 'full' (see _base_covariance), then rotated into the source frame like
+                       LinkInfo::Update (Mapper.h:174-188); measurement noise is drawn from that covariance
+      reversed_frac    fraction of edges stored target -> source, with z and cov of the reversed direction
+      duplicate_frac   fraction of edges repeated as parallel edges with independent noise
+      order            insertion order of the connected nodes: 'chain', 'reversed' or 'shuffled'; the first inserted
+                       node is the solver's anchor, which may then sit anywhere along the chain
+      ids              'dense' (0..N-1) or 'sparse' (unique int32 ids including negative ones and both extremes)
+      world_rotation / world_translation   rigid transform of the whole world (truth and initial guess)
+      isolated_runs    ((fraction, length), ...): runs of consecutive nodes without edges, inserted at that fraction of
+                       the insertion order (never first)
+      detached_nodes   a second walk of that many nodes with its own odometry / loop edges, not connected to the first
+      hub_degree       extra loop edges from the walk's middle node to nodes at least 64 steps away along the walk
+    Returns ids, init, truth (insertion order), edge_a / edge_b (ids), ia / ib (insertion positions), z, cov,
+    component (0 main walk, 1 detached walk, -1 isolated) and anchor (insertion position of the anchor, 0)."""
+    rng = np.random.default_rng(seed)
+    comps = [(0, n_nodes)] + ([(1, detached_nodes)] if detached_nodes else [])
+    truth_l, comp_l, src, dst, kinds = [], [], [], [], []
+    base = 0
+    for cid, n in comps:
+        walk = _lattice_walk(rng, n, lattice, (lattice // 2, lattice // 2) if cid == 0 else (lattice // 4, lattice // 4))
+        th = wrap(walk[:, 2] * (math.pi / 2) + rng.normal(0.0, heading_jitter, n))
+        truth_l.append(np.column_stack([walk[:, 0].astype(float), walk[:, 1].astype(float), th]))
+        comp_l.append(np.full(n, cid))
+        src += list(range(base, base + n - 1)); dst += list(range(base + 1, base + n)); kinds += [0] * (n - 1)
+        site = {}
+        for i in range(n):
+            site.setdefault((int(walk[i, 0]), int(walk[i, 1])), []).append(i)
+        want = n_loops if cid == 0 else max(1, (n_loops * n) // max(n_nodes, 1))
+        pairs, tries = set(), 0
+        while len(pairs) < want and tries < 64 * max(want, 1):
+            tries += 1
+            i = int(rng.integers(n))
+            dx, dy = [(0, 0), (1, 0), (0, 1), (-1, 0), (0, -1)][int(rng.integers(5))]
+            lst = site.get((int(walk[i, 0]) + dx, int(walk[i, 1]) + dy))
+            if lst:
+                j = lst[int(rng.integers(len(lst)))]
+                if abs(j - i) > min_gap:
+                    pairs.add((min(i, j), max(i, j)))
+        for a, b in sorted(pairs):
+            src.append(base + a); dst.append(base + b); kinds.append(1)
+        if cid == 0 and hub_degree:
+            h = n // 2
+            far = np.nonzero(np.abs(np.arange(n) - h) > 64)[0]
+            far = far if len(far) else np.setdiff1d(np.arange(n), [h])
+            for j in rng.choice(far, size=hub_degree, replace=True):
+                src.append(base + h); dst.append(base + int(j)); kinds.append(2)
+        base += n
+    truth = np.concatenate(truth_l)
+    comp = np.concatenate(comp_l)
+    src, dst = np.array(src, dtype=np.int64), np.array(dst, dtype=np.int64)
+    E0 = len(src)
+    dup = np.nonzero(rng.random(E0) < duplicate_frac)[0]
+    src, dst = np.concatenate([src, src[dup]]), np.concatenate([dst, dst[dup]])
+    kinds = np.concatenate([np.array(kinds), np.full(len(dup), 3)])
+    E = len(src)
+    # measurement and covariance of every edge in its forward (walk) direction
+    cov_f = np.empty((E, 3, 3))
+    z_f = _pose_rel(truth[src], truth[dst])
+    for k in range(E):
+        cb = _base_covariance(rng, cov_model, sigma_xy, sigma_th)
+        R = _rot_z(-truth[src[k], 2])
+        cov_f[k] = R @ cb @ R.T
+        z_f[k] += np.linalg.cholesky(cov_f[k]) @ rng.normal(size=3)
+    z_f[:, 2] = wrap(z_f[:, 2])
+    # dead-reckoned initial guess of every walk from its odometry edges (forward direction)
+    init = truth.copy()
+    for k in np.nonzero(kinds == 0)[0]:
+        a, b = src[k], dst[k]
+        c, s = math.cos(init[a, 2]), math.sin(init[a, 2])
+        init[b, 0] = init[a, 0] + c * z_f[k, 0] - s * z_f[k, 1]
+        init[b, 1] = init[a, 1] + s * z_f[k, 0] + c * z_f[k, 1]
+        init[b, 2] = wrap(init[a, 2] + z_f[k, 2])
+    # reversed edges: z^-1 and the covariance pushed through the Jacobian of the inverse
+    z, cov = z_f.copy(), cov_f.copy()
+    rev = np.nonzero(rng.random(E) < reversed_frac)[0]
+    for k in rev:
+        tx, ty, ph = z_f[k]
+        c, s = math.cos(ph), math.sin(ph)
+        z[k] = [-(c * tx + s * ty), -(-s * tx + c * ty), wrap(-ph)]
+        Jinv = np.array([[-c, -s, s * tx - c * ty], [s, -c, c * tx + s * ty], [0.0, 0.0, -1.0]])
+        cov[k] = Jinv @ cov_f[k] @ Jinv.T
+        src[k], dst[k] = dst[k], src[k]
+    cov = 0.5 * (cov + np.transpose(cov, (0, 2, 1)))
+    # world transform
+    if world_rotation or np.any(world_translation):
+        Rw = _rot_z(world_rotation)[:2, :2]
+        t = np.asarray(world_translation, dtype=np.float64)
+        for P in (truth, init):
+            P[:, :2] = P[:, :2] @ Rw.T + t
+            P[:, 2] = wrap(P[:, 2] + world_rotation)
+    # insertion order of the connected nodes, then the isolated runs spliced in
+    nc = len(truth)
+    perm = {"chain": np.arange(nc), "reversed": np.arange(nc)[::-1], "shuffled": rng.permutation(nc)}[order]
+    seq = [("c", int(i)) for i in perm]
+    iso_poses = []
+    for frac, length in sorted(isolated_runs, reverse=True):
+        pos = max(1, min(len(seq), int(round(frac * len(seq)))))
+        run = [("i", len(iso_poses) + k) for k in range(length)]
+        iso_poses += [[rng.uniform(-50, 50), rng.uniform(-50, 50), rng.uniform(-math.pi, math.pi)] for _ in range(length)]
+        seq[pos:pos] = run
+    iso_poses = np.array(iso_poses, dtype=np.float64).reshape(-1, 3)
+    N = len(seq)
+    pos_of = np.empty(nc, dtype=np.int64)
+    out_truth, out_init, out_comp = np.empty((N, 3)), np.empty((N, 3)), np.empty(N, dtype=np.int64)
+    for p, (kind, i) in enumerate(seq):
+        if kind == "c":
+            pos_of[i] = p
+            out_truth[p], out_init[p], out_comp[p] = truth[i], init[i], comp[i]
+        else:
+            out_truth[p] = out_init[p] = iso_poses[i]
+            out_comp[p] = -1
+    if ids == "dense":
+        id_arr = np.arange(N, dtype=np.int32)
+    elif ids == "sparse":
+        lo, hi = np.iinfo(np.int32).min, np.iinfo(np.int32).max
+        pool = np.setdiff1d(np.unique(np.concatenate([[-1, 0], rng.integers(lo + 1, hi, 4 * N + 8)])), [lo, hi])
+        id_arr = rng.permutation(np.concatenate([[lo, hi], rng.permutation(pool)])[:N]).astype(np.int32)
+    else:
+        raise ValueError(f"unknown id scheme {ids!r}")
+    ia, ib = pos_of[src], pos_of[dst]
+    return dict(ids=id_arr, init=out_init, truth=out_truth, edge_a=id_arr[ia], edge_b=id_arr[ib], ia=ia, ib=ib,
+                z=z, cov=cov, component=out_comp, anchor=0)
