@@ -167,6 +167,36 @@ struct TileShared {
 };
 
 // ------------------------------------------------------------------------------------------
+// section timers (build with -DB200_TILE_TIMERS, tools/tile_timers.py): lane 0 of every warp accumulates clock64() deltas
+// per section and adds them to g_tile_timers at the end of the kernel.  Compiled out of the shipped library.
+// ------------------------------------------------------------------------------------------
+#ifdef B200_TILE_TIMERS
+enum { kTmRaster, kTmDesc, kTmCorr, kTmFlush, kTmBarrier, kTmReduce, kTmPair, kTmTotal, kTmCount };
+__device__ unsigned long long g_tile_timers[kTmCount];
+#define TILE_TM_DECL                              \
+  unsigned long long tm_acc[kTmCount] = {};       \
+  long long tm_t = clock64();                     \
+  const long long tm_start = tm_t;
+#define TILE_TM(sec)                                                      \
+  do {                                                                    \
+    const long long tm_now = clock64();                                   \
+    tm_acc[sec] += (unsigned long long)(tm_now - tm_t);                   \
+    tm_t = tm_now;                                                        \
+  } while (0)
+#define TILE_TM_END                                                                 \
+  do {                                                                              \
+    TILE_TM(kTmPair);                                                               \
+    tm_acc[kTmTotal] = (unsigned long long)(tm_t - tm_start);                       \
+    if (lane == 0)                                                                  \
+      for (int s = 0; s < kTmCount; ++s) atomicAdd(&g_tile_timers[s], tm_acc[s]);   \
+  } while (0)
+#else
+#define TILE_TM_DECL
+#define TILE_TM(sec) do {} while (0)
+#define TILE_TM_END do {} while (0)
+#endif
+
+// ------------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------------
 // kPitchW = the sub-grid row pitch in words as a compile-time constant (0 = take it from TileDev): with a constant pitch the 24
@@ -194,6 +224,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
   const int nb = f.nbands;
   const uint32_t bar0 = smem_u32(&sh.bar[0]);
   const uint32_t stg0 = smem_u32(s_raw + f.off_stage);
+  TILE_TM_DECL
 
   if (tid == 0) {
     mbar_init(bar0, 1);
@@ -245,6 +276,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
       mbar_wait(bar0 + 16 + 8 * (iter & 1), (uint32_t)((iter >> 1) & 1));
       cells0 = reinterpret_cast<const int32_t *>(s_raw + f.off_cells + (size_t)(iter & 1) * cell_bytes);
     }
+    TILE_TM(kTmPair);
 
     for (int si = 0; si < nseq; ++si) {
       const TileSeq e = seq[si];
@@ -293,6 +325,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         }
       }
       if (e.flags & (kSeqNewChunk | kSeqNewStage)) __syncthreads();
+      TILE_TM(kTmRaster);
       // ---- prefetch the next descriptor block (this pair's, or the first of this cluster's next pair) ----
       if (tid == 0) {
         const TileSeq * nxt = nullptr;
@@ -301,36 +334,30 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         if (nxt) issue(nxt, (cnt + 1) & 1);
       }
       mbar_wait(bar0 + 8 * (cnt & 1), (cnt >> 1) & 1);
+      TILE_TM(kTmDesc);
       const unsigned char * stg = s_raw + f.off_stage + (size_t)(cnt & 1) * f.stage_bytes;
-      const int32_t * tbl = reinterpret_cast<const int32_t *>(stg);
-      const uint8_t * order = stg + (size_t)e.na * 48;   // (angle, alignment) groups by descending length: the shared queue hands out long items first
-      const uint16_t * pay = reinterpret_cast<const uint16_t *>(stg + (((size_t)e.na * 52 + 15) & ~(size_t)15));
-      // ---- FAST + EDGE beams: warp items (angle, alignment, y-tile, x-tile) from the shared queue ----
-      const int tiles = f.ytiles * f.xtiles;
-      const int nitems = e.na * 4 * tiles;
-      const bool has_edge = (e.flags & kSeqHasEdge) != 0;
+      const uint2 * items = reinterpret_cast<const uint2 *>(stg);   // the host's item list, longest first (format: sm_types.cuh)
+      const uint16_t * pay = reinterpret_cast<const uint16_t *>(stg + (((size_t)e.nitems * 8 + 15) & ~(size_t)15));
+      // ---- FAST + EDGE beams: warp items from the shared queue ----
       for (;;) {
         int item = 0;
         if (lane == 0) item = atomicAdd(&sh.ctr[cnt & 1], 1);
         item = __shfl_sync(0xffffffffu, item, 0);
-        if (item >= nitems) break;
-        const int gi = item / tiles, ti = item - gi * tiles;
-        const int g = order[gi];
-        const int al = g >> 2, m = g & 3;
-        const int yt = ti / f.xtiles, xt = ti - yt * f.xtiles;
+        if (item >= e.nitems) break;
+        const uint2 rec = items[item];
+        int b = (int)(rec.x & 0xFFFFu);
+        const int pe = (int)(rec.x >> 16), me = pe + 2 * (int)(rec.y & 0xFFu);   // plain [b, pe), multi pairs [pe, me)
+        const int al = (int)((rec.y >> 8) & 63u), m = (int)((rec.y >> 14) & 3u);
+        const int xt = (int)((rec.y >> 16) & 63u), yt = (int)((rec.y >> 22) & 255u);
         const int a = e.a0 + al;
         int32_t * Arow = A + (size_t)(a - chunk_a0) * P;
         const int ybase = y_l + kYTile * yt;
        {
-        int b = tbl[(al * 4 + m) * 3 + 0];
-        const int mb = tbl[(al * 4 + m) * 3 + 1], me = tbl[(al * 4 + m) * 3 + 2];
-        const int pe = mb;   // plain entries [b, pe) (list start 4-aligned), multi entries (offset, multiplicity) pairs [mb, me)
         int eb = 0, ee = 0;
-        if (has_edge) {
+        if (rec.y >> 31) {
           const int32_t * es = f.edge_start + (((size_t)q * nA + a) * 4 * nb + e.stage) * 4 + m;
           eb = es[0]; ee = es[1];
         }
-        if (b == pe && mb == me && eb == ee) break;   // the groups are sorted by length: every later item is empty too
         uint32_t base = smem_u32(S8) + (uint32_t)(((y_l + kYTile * yt) * pitch_w + 4 * xt + j_l) * 4);   // shared-window address
         asm volatile("" : "+r"(base));   // one opaque register: every descriptor then costs PRMT + IMAD (no re-association of the sum)
         // Idle lanes of the last y-tile (rows beyond the last pose) read past the band's nY-row halo, at most 47 rows into the
@@ -338,10 +365,11 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         // so a band needs a halo of nY rows, not of whole y-tiles, and the row offsets stay warp-uniform (LDS [R + UR]).
         const int x0 = 4 * (4 * xt + j_l) - m;
         auto flush = [&](const uint32_t (&T0)[kRowTiles], const uint32_t (&T1)[kRowTiles]) {
+          TILE_TM(kTmCorr);
           uint32_t any = 0;
 #pragma unroll
           for (int r = 0; r < kRowTiles; ++r) any |= T0[r] | T1[r];
-          if (!__any_sync(0xffffffffu, any != 0)) return;
+          if (!__any_sync(0xffffffffu, any != 0)) { TILE_TM(kTmFlush); return; }
 #pragma unroll
           for (int r = 0; r < kRowTiles; ++r) {
             const int y = ybase + 8 * r;
@@ -353,68 +381,63 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
             if (v2 && (unsigned)(x0 + 2) < (unsigned)nX) atomicAdd(dst + 2, v2);
             if (v3 && (unsigned)(x0 + 3) < (unsigned)nX) atomicAdd(dst + 3, v3);
           }
+          TILE_TM(kTmFlush);
         };
-        bool multi_done = (mb == me);
-        if (b < pe || !multi_done) {
-          do {
-            const int ce = min(pe, b + kChunkBeams);
-            uint32_t T0[kRowTiles], T1[kRowTiles];
+        // an item's plain and multi beams weigh at most kChunkBeams (the host splits longer groups): one flush
+        if (b < me) {
+          uint32_t T0[kRowTiles], T1[kRowTiles];
 #pragma unroll
-            for (int r = 0; r < kRowTiles; ++r) { T0[r] = 0; T1[r] = 0; }
-            for (; b + 3 < ce; b += 4) {   // 4 beams: one broadcast LDS.64 of descriptors, two byte-wise pair sums, one 3-input add per field
-              const uint2 dd = *reinterpret_cast<const uint2 *>(pay + b);
-              // 16-bit word offsets -> byte addresses: one PRMT (half-word extract) + one shift-add each
-              const uint32_t o0 = base + 4u * __byte_perm(dd.x, 0, 0x4410), o1 = base + 4u * __byte_perm(dd.x, 0, 0x4432);
-              const uint32_t o2 = base + 4u * __byte_perm(dd.y, 0, 0x4410), o3 = base + 4u * __byte_perm(dd.y, 0, 0x4432);
+          for (int r = 0; r < kRowTiles; ++r) { T0[r] = 0; T1[r] = 0; }
+          for (; b + 3 < pe; b += 4) {   // 4 beams: one broadcast LDS.64 of descriptors, two byte-wise pair sums, one 3-input add per field
+            const uint2 dd = *reinterpret_cast<const uint2 *>(pay + b);
+            // 16-bit word offsets -> byte addresses: one PRMT (half-word extract) + one shift-add each
+            const uint32_t o0 = base + 4u * __byte_perm(dd.x, 0, 0x4410), o1 = base + 4u * __byte_perm(dd.x, 0, 0x4432);
+            const uint32_t o2 = base + 4u * __byte_perm(dd.y, 0, 0x4410), o3 = base + 4u * __byte_perm(dd.y, 0, 0x4432);
 #pragma unroll
-              for (int r = 0; r < kRowTiles; ++r) {
-                const uint32_t wa = lds_u32(o0 + r * 8 * pitchB) +
-                                    lds_u32(o1 + r * 8 * pitchB);
-                const uint32_t wb = lds_u32(o2 + r * 8 * pitchB) +
-                                    lds_u32(o3 + r * 8 * pitchB);
-                T0[r] = T0[r] + even_bytes_t(wa) + even_bytes_t(wb);
-                T1[r] = T1[r] + odd_bytes_t(wa) + odd_bytes_t(wb);
-              }
+            for (int r = 0; r < kRowTiles; ++r) {
+              const uint32_t wa = lds_u32(o0 + r * 8 * pitchB) +
+                                  lds_u32(o1 + r * 8 * pitchB);
+              const uint32_t wb = lds_u32(o2 + r * 8 * pitchB) +
+                                  lds_u32(o3 + r * 8 * pitchB);
+              T0[r] = T0[r] + even_bytes_t(wa) + even_bytes_t(wb);
+              T1[r] = T1[r] + odd_bytes_t(wa) + odd_bytes_t(wb);
             }
-            for (; b + 1 < ce; b += 2) {
-              const uint32_t dd = *reinterpret_cast<const uint32_t *>(pay + b);
-              const uint32_t o0 = base + ((dd & 0xFFFFu) << 2), o1 = base + ((dd >> 16) << 2);
+          }
+          for (; b + 1 < pe; b += 2) {
+            const uint32_t dd = *reinterpret_cast<const uint32_t *>(pay + b);
+            const uint32_t o0 = base + ((dd & 0xFFFFu) << 2), o1 = base + ((dd >> 16) << 2);
 #pragma unroll
-              for (int r = 0; r < kRowTiles; ++r) {
-                const uint32_t w = lds_u32(o0 + r * 8 * pitchB) +
-                                   lds_u32(o1 + r * 8 * pitchB);
-                T0[r] += even_bytes_t(w);
-                T1[r] += odd_bytes_t(w);
-              }
+            for (int r = 0; r < kRowTiles; ++r) {
+              const uint32_t w = lds_u32(o0 + r * 8 * pitchB) +
+                                 lds_u32(o1 + r * 8 * pitchB);
+              T0[r] += even_bytes_t(w);
+              T1[r] += odd_bytes_t(w);
             }
-            if (b < ce) {
-              const uint32_t o0 = base + ((uint32_t)pay[b] << 2);
+          }
+          if (b < pe) {
+            const uint32_t o0 = base + ((uint32_t)pay[b] << 2);
 #pragma unroll
-              for (int r = 0; r < kRowTiles; ++r) {
-                const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
-                T0[r] += even_bytes_t(w);
-                T1[r] += odd_bytes_t(w);
-              }
-              ++b;
+            for (int r = 0; r < kRowTiles; ++r) {
+              const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
+              T0[r] += even_bytes_t(w);
+              T1[r] += odd_bytes_t(w);
             }
-            if (b == pe && !multi_done) {
-              // beams that share one grid cell: one load, fields times k (the host only builds multi entries when the
-              // whole group's weight fits one flush)
-              for (int k = mb; k < me; k += 2) {
-                const uint32_t dm = *reinterpret_cast<const uint32_t *>(pay + k);
-                const uint32_t o0 = base + ((dm & 0xFFFFu) << 2);
-                const uint32_t kk = dm >> 16;
+            ++b;
+          }
+          // beams that share one grid cell: one load, fields times k (the host only builds multi entries when the whole
+          // group's weight fits one flush)
+          for (int k = pe; k < me; k += 2) {
+            const uint32_t dm = *reinterpret_cast<const uint32_t *>(pay + k);
+            const uint32_t o0 = base + ((dm & 0xFFFFu) << 2);
+            const uint32_t kk = dm >> 16;
 #pragma unroll
-                for (int r = 0; r < kRowTiles; ++r) {
-                  const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
-                  T0[r] += even_bytes_t(w) * kk;
-                  T1[r] += odd_bytes_t(w) * kk;
-                }
-              }
-              multi_done = true;
+            for (int r = 0; r < kRowTiles; ++r) {
+              const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
+              T0[r] += even_bytes_t(w) * kk;
+              T1[r] += odd_bytes_t(w) * kk;
             }
-            flush(T0, T1);
-          } while (b < pe || !multi_done);
+          }
+          flush(T0, T1);
         }
         // EDGE beams of this group (window partly outside the grid): the same word loads with rows / words outside the
         // band allocation masked (they index outside [0, data_size) or wrap in the reference; the wrapped part is added
@@ -445,6 +468,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         }
        }
       }
+      TILE_TM(kTmCorr);
       if (e.flags & kSeqNewStage) {
         // ---- wrapped part of EDGE beams (row parity flipped list): poses whose column left [0, stride) by less than a
         //      stride read the neighbouring row at column -/+ stride (linear index, M.cpp:1192-1200) ----
@@ -497,6 +521,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
       if (tid == 0) sh.ctr[(cnt + 1) & 1] = 0;
       __syncthreads();
       ++cnt;
+      TILE_TM(kTmBarrier);
 
       if (e.flags & kSeqEndChunk) {
         // ================= chunk reduction: per-cell max image, best response, ordered tie list =================
@@ -572,6 +597,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         }
         first_chunk = false;
         __syncthreads();
+        TILE_TM(kTmReduce);
       }
     }
 
@@ -698,6 +724,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
     }
   }
   if (pending_wait) cluster_wait();   // nobody leaves while a leader may still read its shared memory
+  TILE_TM_END;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -727,6 +754,36 @@ static inline bool d_max_n_ok(int max_n) { return max_n > 0 && (max_n & 3) == 0 
 
 static inline int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
+// The warp items of one descriptor block, longest first (the shared queue then hands out long items first).  tbl holds (plain
+// begin, multi begin, multi end) per (angle, alignment) group, nedge the group's EDGE beams.  A group's plain list is cut into
+// pieces of at most kChunkBeams beams (4-aligned starts: the 4-beam step reads descriptors with 64-bit loads), so that every item
+// flushes its 16-bit fields once; the multi pairs and the EDGE beams go with the last piece.
+static void build_block_items(const std::vector<int32_t> & tbl, const std::vector<int> & nedge, int na, int xtiles, int ytiles,
+                              std::vector<uint2> & out)
+{
+  struct Piece { int work; int pb, pe, mpairs, al, m; bool edge; };
+  std::vector<Piece> pieces;
+  for (int g = 0; g < na * 4; ++g) {
+    const int pb = tbl[3 * g], mb = tbl[3 * g + 1], mpairs = (tbl[3 * g + 2] - mb) / 2, ne = nedge[g];
+    if (mb == pb && mpairs == 0 && ne == 0) continue;
+    for (int s = pb;; s += kChunkBeams) {
+      Piece p{0, s, std::min(mb, s + kChunkBeams), 0, g >> 2, g & 3, false};
+      if (p.pe == mb) { p.mpairs = mpairs; p.edge = ne > 0; }
+      p.work = (p.pe - p.pb) + p.mpairs + (p.edge ? ne : 0);
+      pieces.push_back(p);
+      if (p.pe == mb) break;
+    }
+  }
+  std::stable_sort(pieces.begin(), pieces.end(), [](const Piece & x, const Piece & y) { return x.work > y.work; });
+  out.clear();
+  for (const Piece & p : pieces)
+    for (int yt = 0; yt < ytiles; ++yt)
+      for (int xt = 0; xt < xtiles; ++xt)
+        out.push_back(make_uint2((uint32_t)p.pb | ((uint32_t)p.pe << 16),
+                                 (uint32_t)p.mpairs | ((uint32_t)p.al << 8) | ((uint32_t)p.m << 14) | ((uint32_t)xt << 16) |
+                                   ((uint32_t)yt << 22) | (p.edge ? 0x80000000u : 0u)));
+}
+
 bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
 {
   const GridGeom & g = h->g;
@@ -747,6 +804,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   int pitch_w = (g.stride / 2 + 16 + 3) / 4;             // sub-grid row + the 3-word overhang of the last x-tile
   while ((pitch_w & 7) != 4) ++pitch_w;                  // 8 rows x 4 words of a warp hit 32 distinct banks
   const int xtiles = (nX + 3 + 15) / 16, ytiles = (nY + kYTile - 1) / kYTile;
+  if (xtiles > kItemMaxXTiles || ytiles > kItemMaxYTiles) return bail(9);
   const int rows_valid = (g.height + 1) / 2;
   const int halo = nY + 2;                               // rows a beam window reaches below its base row (idle row tiles are clamped) + the wrapped row
   const int base_rows = std::max(1, rows_valid - nY + 1);   // distinct base rows of beams whose window is inside the grid
@@ -775,8 +833,8 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     const int nAc = (nA + V - 1) / V;
     if ((nA + nAc - 1) / nAc != V || nAc > 63) continue;   // same chunk size as a smaller V; group ids are bytes
     const int a_bytes = (nAc * P * 4 + 15) & ~15;
-    // staging buffer: header + 1.5 x the average descriptor bytes of a (chunk, phase) block, at least one angle's worst case
-    const int one_angle = 52 + 2 * n + 64;
+    // staging buffer: item list + 1.5 x the average descriptor bytes of a (chunk, phase) block, at least one angle's worst case
+    const int one_angle = 32 * xtiles * ytiles + 2 * n + 64;   // + one item record per (alignment, tile)
     int stage = 16 + nAc * 52 + (nAc * n * 2 * 3) / 8 + 64 * nAc;
     stage = std::max(stage, one_angle + 64);
     stage = (stage + 127) & ~127;
@@ -951,6 +1009,8 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
       }
     std::vector<uint16_t> pay;
     std::vector<int32_t> tbl;
+    std::vector<int> nedge;
+    std::vector<uint2> items;
     for (int r = 0; r < C; ++r) {
       seq_start[(size_t)q * C + r] = (int32_t)seq.size();
       for (int v = r; v < V; v += C) {
@@ -961,47 +1021,39 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
           bool first_sub = true;
           do {
             tbl.clear(); pay.clear();
-            int na = 0;
+            int na = 0, npieces = 0;   // pieces of the block's groups so far (items = pieces x tiles)
             while (a + na < ca0 + cna) {
               const Encoded & E = enc[(size_t)(a + na) * nstage + sg];
-              const size_t hdr = (((size_t)(na + 1) * 52) + 15) & ~(size_t)15;
+              int ep = 0;
+              for (int m = 0; m < 4; ++m) ep += std::max(1, (E.tbl[3 * m + 1] - E.tbl[3 * m] + kChunkBeams - 1) / kChunkBeams);
+              const size_t hdr = (((size_t)(npieces + ep) * xtiles * ytiles * 8) + 15) & ~(size_t)15;
               const size_t bytes = (hdr + (pay.size() + E.pay.size()) * 2 + 15) & ~(size_t)15;
-              if (bytes > (size_t)stage_bytes) {
+              if (bytes > (size_t)stage_bytes || pay.size() + E.pay.size() > 65535) {   // item ranges are 16-bit
                 if (na > 0) break;
                 return bail(8);   // one angle does not fit the staging buffer
               }
               const int shift = (int)pay.size();
               for (int k = 0; k < 12; ++k) tbl.push_back(E.tbl[k] + shift);
               pay.insert(pay.end(), E.pay.begin(), E.pay.end());
+              npieces += ep;
               ++na;
             }
-            const size_t hdr = (((size_t)na * 52) + 15) & ~(size_t)15;
+            nedge.assign((size_t)na * 4, 0);
+            for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)egrp[((size_t)(a + (g2 >> 2)) * nstage + sg) * 4 + (g2 & 3)].size();
+            build_block_items(tbl, nedge, na, xtiles, ytiles, items);
+            const size_t hdr = ((items.size() * 8) + 15) & ~(size_t)15;
             const size_t bytes = std::max<size_t>(16, (hdr + pay.size() * 2 + 15) & ~(size_t)15);
             TileSeq e{};
             e.off = (int32_t)blob.size();
             e.bytes = (int32_t)bytes;
-            e.chunk = (int16_t)v; e.stage = (int16_t)sg; e.a0 = (int16_t)a; e.na = (int16_t)na;
+            e.chunk = (int16_t)v; e.stage = (int16_t)sg; e.a0 = (int16_t)a; e.nitems = (int16_t)items.size();
             e.flags = (first_sub ? kSeqNewStage : 0u) | ((first_sub && sg == 0) ? kSeqNewChunk : 0u);
-            for (int aa = a; aa < a + na; ++aa)
-              for (int m = 0; m < 4; ++m)
-                if (!egrp[((size_t)aa * nstage + sg) * 4 + m].empty()) e.flags |= kSeqHasEdge;
             if (first_sub)
               for (int aa = ca0; aa < ca0 + cna; ++aa)
                 if (!wgrp[(size_t)aa * nstage + sg].empty()) e.flags |= kSeqHasWrap;
             blob.resize(blob.size() + bytes, 0);
-            if (na > 0) {
-              // (angle, alignment) groups by descending work: plain + multi descriptors + edge entries
-              std::vector<std::pair<int, int>> wt;
-              for (int g2 = 0; g2 < na * 4; ++g2) {
-                const int w = (tbl[3 * g2 + 1] - tbl[3 * g2]) + (tbl[3 * g2 + 2] - tbl[3 * g2 + 1]) / 2 +
-                              (int)egrp[((size_t)(a + (g2 >> 2)) * nstage + sg) * 4 + (g2 & 3)].size();
-                wt.emplace_back(-w, g2);
-              }
-              std::sort(wt.begin(), wt.end());
-              for (int g2 = 0; g2 < na * 4; ++g2) blob[e.off + (size_t)na * 48 + g2] = (uint8_t)wt[g2].second;
-              std::memcpy(blob.data() + e.off, tbl.data(), tbl.size() * 4);
-              if (!pay.empty()) std::memcpy(blob.data() + e.off + hdr, pay.data(), pay.size() * 2);
-            }
+            if (!items.empty()) std::memcpy(blob.data() + e.off, items.data(), items.size() * 8);
+            if (!pay.empty()) std::memcpy(blob.data() + e.off + hdr, pay.data(), pay.size() * 2);
             seq.push_back(e);
             a += na;
             first_sub = false;
@@ -1082,3 +1134,19 @@ void launch_sweep_tile(b200sm * h, SweepHost & S, cudaStream_t st)
 }
 
 }  // namespace b200
+
+#ifdef B200_TILE_TIMERS
+// section totals of the instrumented build, in the order of the kTm* enum: copied to out (when non-null), then zeroed when
+// reset != 0.  Returns the number of sections, or -1 on a CUDA error.
+extern "C" int b200_tile_timers(unsigned long long * out, int reset)
+{
+  using namespace b200;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  if (out && cudaMemcpyFromSymbol(out, g_tile_timers, sizeof(g_tile_timers)) != cudaSuccess) return -1;
+  if (reset) {
+    const unsigned long long zero[kTmCount] = {};
+    if (cudaMemcpyToSymbol(g_tile_timers, zero, sizeof(zero)) != cudaSuccess) return -1;
+  }
+  return kTmCount;
+}
+#endif

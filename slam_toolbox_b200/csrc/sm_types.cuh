@@ -151,10 +151,17 @@ struct TileSeq {                 // one descriptor block of a query's schedule (
   int32_t off;                   // byte offset in the descriptor blob (16-byte aligned)
   int32_t bytes;                 // size, multiple of 16
   int16_t chunk, stage;          // angle chunk; stage = phase * nbands + band
-  int16_t a0, na;                // angles [a0, a0 + na) of this block (global indices)
+  int16_t a0;                    // first angle of this block (global index)
+  int16_t nitems;                // warp items of this block (8-byte records at the start of the block, see below)
   uint32_t flags;                // kSeq* bits
 };
-constexpr uint32_t kSeqNewChunk = 1, kSeqNewStage = 2, kSeqEndChunk = 4, kSeqHasEdge = 8, kSeqHasWrap = 16;
+// One warp item of a descriptor block (8 bytes, longest first): beams [pb, pe) of the payload's plain list and the
+// mpairs (offset, multiplicity) pairs that follow them, for the angle a0 + al, alignment m and tile (xt, yt).  Items of a
+// long group hold consecutive pieces of its plain list; the EDGE beams of a (group, tile) go with exactly one item (edge).
+//   x = pb | pe << 16;  y = mpairs | al << 8 | m << 14 | xt << 16 | yt << 22 | edge << 31
+// (al < 64: the planner's nAc <= 63; mpairs < 256: multi entries exist only in groups of at most kChunkBeams beams)
+constexpr int kItemMaxXTiles = 64, kItemMaxYTiles = 256;
+constexpr uint32_t kSeqNewChunk = 1, kSeqNewStage = 2, kSeqEndChunk = 4, kSeqHasWrap = 16;
 struct TileDev {
   int enabled;
   int C, V, nAc;                 // cluster size, angle chunks, angles per chunk
