@@ -166,6 +166,11 @@ int b200sm_batch_info(b200sm * h, int32_t info[8]);
 /* Plan of the tiled cluster kernel for the uploaded sweep: info = {available, cluster size (CTAs per pair), angle chunks,
  * sub-grid bands per parity phase, rows per band, refusal reason, resident clusters, shared memory per CTA (KB)}. */
 int b200sm_batch_tile_info(b200sm * h, int32_t info[8]);
+/* What the tiled kernel's descriptor blocks hold for the uploaded sweep (host-side counts, zero when the tiled kernel was
+ * refused): stats = {descriptor blocks, continuation sub-blocks (a stage's angles split over several staging buffers), largest
+ * EDGE group (beams), (angle, phase, band, alignment) groups cut into more than one item, multi entries (cell, multiplicity),
+ * largest multiplicity, largest plain group (beams), wrap2 entries}. */
+int b200sm_batch_tile_stats(b200sm * h, int32_t stats[8]);
 /* How the last fetch finished its pairs: stats = {pairs whose volume was all zero (all poses tie: closed form, once per
  * query; with use_response_expansion: pairs with an empty raster, closed form of the widest expansion pass), pairs handed one by one to the single-match path (tie list overflow with a non-zero best, response expansion),
  * pairs, 0}. */

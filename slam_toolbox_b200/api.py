@@ -112,6 +112,7 @@ def lib():
     L.b200sm_batch_winner_records.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
     L.b200sm_batch_winners_select.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int64), _DP, _DP, _DP]
     L.b200sm_batch_tile_info.argtypes = [C.c_void_p, _IP]
+    L.b200sm_batch_tile_stats.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_fetch_stats.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_upload_timing.argtypes = [C.c_void_p, _DP]
     L.b200sm_batch_reduce_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
@@ -390,6 +391,13 @@ class ScanMatcher:
         _check(lib().b200sm_batch_tile_info(self._h, _ip(info)))
         return dict(available=bool(info[0]), cluster=int(info[1]), chunks=int(info[2]), bands=int(info[3]), band_rows=int(info[4]),
                     refused_reason=int(info[5]), clusters=int(info[6]), smem_kb=int(info[7]))
+
+    def batch_tile_stats(self):
+        """What the tiled kernel's descriptor blocks hold for the uploaded sweep (b200sm_batch_tile_stats)."""
+        st = np.zeros(8, dtype=np.int32)
+        _check(lib().b200sm_batch_tile_stats(self._h, _ip(st)))
+        return dict(blocks=int(st[0]), sub_blocks=int(st[1]), max_edge_group=int(st[2]), split_groups=int(st[3]),
+                    multi_entries=int(st[4]), max_multiplicity=int(st[5]), max_plain_group=int(st[6]), wrap2_entries=int(st[7]))
 
     def batch_upload_timing(self):
         t = np.zeros(3)

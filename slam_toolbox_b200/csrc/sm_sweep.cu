@@ -1530,6 +1530,13 @@ int b200sm_batch_tile_info(b200sm * h, int32_t info[8])
   return B200_OK;
 }
 
+int b200sm_batch_tile_stats(b200sm * h, int32_t stats[8])
+{
+  if (!h || !stats || !h->sweep.uploaded) return B200_ERR_INVALID_ARG;
+  for (int i = 0; i < 8; ++i) stats[i] = h->sweep.tile_stats[i];
+  return B200_OK;
+}
+
 int b200sm_batch_fetch_stats(b200sm * h, int32_t stats[4])
 {
   if (!h || !stats) return B200_ERR_INVALID_ARG;

@@ -792,8 +792,13 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   TileDev & T = S.tile;
   T = TileDev{};
   for (int i = 0; i < 8; ++i) S.tile_info[i] = 0;
-  auto bail = [&](int why) { S.tile_info[5] = why; return false; };
-  if (g.order_dependent) return bail(1);                 // AddScan's occupancy test makes the raster sequential (generic kernel)
+  for (int i = 0; i < 8; ++i) S.tile_stats[i] = 0;
+  auto bail = [&](int why) {
+    for (int i = 0; i < 8; ++i) S.tile_stats[i] = 0;
+    S.tile_info[5] = why;
+    return false;
+  };
+  if (g.order_dependent) return bail(1);                // AddScan's occupancy test makes the raster sequential (generic kernel)
   if ((g.stride & 1) || nA < 1 || nA > 4096) return bail(2);
   for (int q = 0; q < nq; ++q) {
     const CorrPlan & pl = S.plans[q];
@@ -833,8 +838,10 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     const int nAc = (nA + V - 1) / V;
     if ((nA + nAc - 1) / nAc != V || nAc > 63) continue;   // same chunk size as a smaller V; group ids are bytes
     const int a_bytes = (nAc * P * 4 + 15) & ~15;
-    // staging buffer: item list + 1.5 x the average descriptor bytes of a (chunk, phase) block, at least one angle's worst case
-    const int one_angle = 32 * xtiles * ytiles + 2 * n + 64;   // + one item record per (alignment, tile)
+    // staging buffer: item list + 1.5 x the average descriptor bytes of a (chunk, phase) block, at least one angle's worst case:
+    // one item record per (alignment, tile), plus one per tile for every further kChunkBeams-piece of a long group -- the
+    // groups of one angle hold at most n beams, so they are cut at most (n - 1) / kChunkBeams more times
+    const int one_angle = 8 * xtiles * ytiles * (4 + std::max(n - 1, 0) / kChunkBeams) + 2 * n + 64;
     int stage = 16 + nAc * 52 + (nAc * n * 2 * 3) / 8 + 64 * nAc;
     stage = std::max(stage, one_angle + 64);
     stage = (stage + 127) & ~127;
@@ -1041,6 +1048,17 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
             nedge.assign((size_t)na * 4, 0);
             for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)egrp[((size_t)(a + (g2 >> 2)) * nstage + sg) * 4 + (g2 & 3)].size();
             build_block_items(tbl, nedge, na, xtiles, ytiles, items);
+            int32_t * ts = S.tile_stats;
+            ts[0] += 1;
+            ts[1] += first_sub ? 0 : 1;
+            for (int g2 = 0; g2 < na * 4; ++g2) {
+              const int pb = tbl[3 * g2], mb = tbl[3 * g2 + 1], me = tbl[3 * g2 + 2];
+              ts[2] = std::max(ts[2], nedge[g2]);
+              ts[3] += mb - pb > kChunkBeams ? 1 : 0;
+              ts[4] += (me - mb) / 2;
+              for (int k = mb; k < me; k += 2) ts[5] = std::max(ts[5], (int32_t)pay[k + 1]);
+              ts[6] = std::max(ts[6], mb - pb);
+            }
             const size_t hdr = ((items.size() * 8) + 15) & ~(size_t)15;
             const size_t bytes = std::max<size_t>(16, (hdr + pay.size() * 2 + 15) & ~(size_t)15);
             TileSeq e{};
@@ -1066,6 +1084,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   seq_start[(size_t)nq * C] = (int32_t)seq.size();
   edge_start[(size_t)nq * nA * nstage * 4] = (int32_t)edge.size();
   wrap2_start[(size_t)nq * nA * nstage] = (int32_t)wrap2.size();
+  S.tile_stats[7] = (int32_t)wrap2.size();
   edge.push_back(0); wrap2.push_back(0); slow.push_back(0);
   blob.resize(blob.size() + 16, 0);
 

@@ -213,6 +213,9 @@ struct SweepHost {
   size_t tile_smem = 0;
   int tile_grid = 0;
   int32_t tile_info[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // enabled, C, V, nbands, band rows, refusal reason, clusters, smem KB
+  // what the tiled kernel's descriptor blocks contain (b200sm_batch_tile_stats): blocks, continuation sub-blocks, largest EDGE
+  // group, groups cut into pieces, multi entries, largest multiplicity, largest plain group, wrap2 entries
+  int32_t tile_stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   DevBuf<uint8_t> d_tile_desc;
   DevBuf<TileSeq> d_tile_seq;
   DevBuf<int32_t> d_tile_seq_start, d_tile_edge, d_tile_edge_start, d_tile_wrap2, d_tile_wrap2_start, d_tile_slow, d_tile_slow_start;

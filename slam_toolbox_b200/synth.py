@@ -511,3 +511,89 @@ def make_pose_graph_family(seed: int, n_nodes: int = 2000, n_loops: int = 4000, 
     ia, ib = pos_of[src], pos_of[dst]
     return dict(ids=id_arr, init=out_init, truth=out_truth, edge_a=id_arr[ia], edge_b=id_arr[ib], ia=ia, ib=ib,
                 z=z, cov=cov, component=out_comp, anchor=0)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Adversarial inputs for the batched sweep kernels: beams piled into one grid cell, tied best poses, very long queries.
+# Each query and candidate block carries its own laser geometry (angle_min, angle_increment).
+# ---------------------------------------------------------------------------------------------------------------------------
+@dataclass
+class AdversarialSweep:
+    query_ranges: np.ndarray          # (Q, n)
+    query_poses: np.ndarray           # (Q, 3)
+    cand_ranges: np.ndarray           # (S, m)
+    cand_poses: np.ndarray            # (S, 3)
+    chain_start: np.ndarray           # (C+1,)
+    query_laser: tuple = (ANGLE_MIN, ANGLE_INC)
+    cand_laser: tuple = (ANGLE_MIN, ANGLE_INC)
+
+
+DENSE_INC = 1e-9   # rad: a cluster of 2000 beams at 13 m spans 26 um, so it sits in one 5 cm cell at every search angle
+
+
+def make_dense_sweep(clusters=(640,), *, edge: bool = False, n_chains: int = 2, seed: int = 101) -> AdversarialSweep:
+    """One query whose beams pile up in a few grid cells: cluster i is clusters[i] beams at one range, fanned over a few
+    nano-radians, so every search angle puts the whole cluster in one cell (one descriptor group of that many beams).
+    Candidates are room scans of make_loop_sweep around the query plus, per cluster, a scan from the query's pose that draws a
+    ring at the cluster's range (so that the cluster's cell is occupied near the zero-offset pose).
+
+    edge=True puts the clusters 12.3 m (and further) behind the query along -x: their pose window leaves the correlation grid
+    (range threshold 12 m) through its left side, so they are EDGE beams with row-wrapped (wrap2) entries."""
+    ls = make_loop_sweep(seed, n_queries=1, n_chains=n_chains, chain_len=1)
+    q = ls.query_poses[0].copy()
+    if edge:
+        q[2] = math.pi
+        radii = [12.3 + 0.35 * i for i in range(len(clusters))]
+    else:
+        radii = [0.55 + 0.35 * i for i in range(len(clusters))]
+    qr = np.concatenate([np.full(k, r) for k, r in zip(clusters, radii)])
+    rings = np.array([np.full(N_BEAMS, r) for r in radii])
+    cr = np.concatenate([ls.cand_ranges, rings])
+    cp = np.concatenate([ls.cand_poses, np.repeat(q[None, :], len(radii), axis=0)])
+    chain_start = np.append(np.arange(n_chains + 1), len(cr)).astype(np.int32)   # one room scan per chain, then the rings
+    return AdversarialSweep(qr[None, :], q[None, :], cr, cp, chain_start, (0.0, DENSE_INC), (ANGLE_MIN, ANGLE_INC))
+
+
+# Query beams (index into the 1081-beam laser, range in m) whose coarse volume against make_tie_sweep's one-point candidate has
+# exactly k maximal poses (response 1/1081), on the 4 m / 0.05 m grid with +-20 deg at 2 deg.  Found once with the oracle; pinned
+# by tests/test_sweep_fixtures.py.
+TIE_BEAMS = {
+    1: ((770, 0.15),),
+    2: ((536, 0.15),),
+    23: ((16, 0.3), (224, 1.9), (640, 1.9), (1069, 0.3)),
+    24: ((107, 0.5), (172, 1.9), (237, 1.6), (744, 0.5)),
+    25: ((367, 1.9), (601, 0.5), (770, 0.15), (848, 1.6), (939, 1.6), (1056, 1.6)),
+    100: ((55, 0.15), (68, 1.6), (81, 1.9), (120, 1.6), (198, 1.6), (302, 0.3), (432, 1.9), (536, 0.5), (705, 0.3), (757, 1.9),
+          (809, 0.5), (848, 1.9), (887, 1.6), (913, 0.3), (965, 1.9), (1043, 0.5)),
+}
+TIE_POSE = (10.0, 12.0, 0.3)
+TIE_CAND_LASER = (0.0, 0.5 * math.pi)
+TIE_CAND_RANGES = (0.3, 5.0)   # FindValidPoints keeps the first reading only: one occupied cell, 0.3 m ahead of the query
+
+
+def make_tie_sweep(ks=(1, 2, 23, 24, 25, 100), n_cands: int = 1) -> AdversarialSweep:
+    """Queries with a few finite readings (the rest inf) against a candidate that rasterises to a single occupied cell: every
+    pose that puts one reading on that cell scores 100, nothing scores more, and the readings are far enough apart that no pose
+    puts two of them near it.  Query i has exactly ks[i] tied best poses, spread over the angles.  n_cands identical candidates,
+    one per chain."""
+    qr = np.full((len(ks), N_BEAMS), np.inf)
+    for row, k in enumerate(ks):
+        for i, d in TIE_BEAMS[k]:
+            qr[row, i] = d
+    qp = np.repeat(np.array([TIE_POSE]), len(ks), axis=0)
+    cr = np.repeat(np.array([TIE_CAND_RANGES]), n_cands, axis=0)
+    cp = np.repeat(np.array([TIE_POSE]), n_cands, axis=0)
+    return AdversarialSweep(qr, qp, cr, cp, np.arange(n_cands + 1, dtype=np.int32), (ANGLE_MIN, ANGLE_INC), TIE_CAND_LASER)
+
+
+def make_long_query_sweep(n: int, seed: int = 7, n_chains: int = 3, inf_frac: float = 0.97) -> AdversarialSweep:
+    """One query of n beams over the usual 270 deg field of view (a room scan at n / 1081 times the angular density, a fraction
+    inf_frac of the readings replaced by inf) and n_chains room-scan candidates.  With the defaults, n = 10240 and the 4 m /
+    0.05 m grid with a 0.05 m smear (5 x 5 kernel) at +-2 deg / 2 deg, chain 1's best two integer sums are s and s - 1: their
+    responses differ by 1 / (100 n) < 1e-6, so both count as ties of the best."""
+    ls = make_loop_sweep(seed, n_queries=1, n_chains=n_chains, chain_len=1)
+    inc = (ANGLE_MAX - ANGLE_MIN) / (n - 1)
+    rng = np.random.default_rng(seed)
+    qr = noisy(raycast(ls.world, ls.query_true, n_beams=n, angle_inc=inc), rng)
+    qr[:, rng.random(n) < inf_frac] = np.inf
+    return AdversarialSweep(qr, ls.query_poses, ls.cand_ranges, ls.cand_poses, ls.chain_start, (ANGLE_MIN, inc), (ANGLE_MIN, ANGLE_INC))
