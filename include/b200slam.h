@@ -117,7 +117,11 @@ int b200sm_grid_copy(b200sm * h, uint8_t * out, int32_t cap);
  *   chain_start[0..nchains]     chain j = scans[chain_start[j] .. chain_start[j+1])
  *   pair_query/pair_chain[np]   pairs to match; both NULL = all nq*nchains pairs, query-major
  * Outputs per pair p: response[p], mean[3p..], cov[9p..]  -- identical to calling
- * b200sm_match(h, &queries[pair_query[p]], chain pair_chain[p], ...) one by one. */
+ * b200sm_match(h, &queries[pair_query[p]], chain pair_chain[p], ...) one by one.
+ * Bounds (this call and b200sm_batch_upload / _run below): any angle window; a query may have up to
+ * 51,200 readings (one lookup row of n int32 must fit 200 KB of shared memory; more -> upload returns
+ * B200_ERR_UNSUPPORTED); a candidate scan up to 12,044 readings (FindValidPoints stages 17 B per point in
+ * 200 KB of shared memory; more -> run returns B200_ERR_UNSUPPORTED). */
 int b200sm_match_batch(b200sm * h, const b200_scan * queries, int32_t nq, const b200_scan * scans,
                        int32_t nscans, const int32_t * chain_start, int32_t nchains,
                        const int32_t * pair_query, const int32_t * pair_chain, int32_t npairs,

@@ -222,10 +222,14 @@ __device__ void pair_epilogue(const SweepDev & d, int pair, int q, const SumAt s
 // of every valid point (AddScan, M.cpp:1080-1104), correlate all (x, y, theta) poses against it
 // (M.cpp:641-694 + 1172-1208) and reduce (pair_epilogue).  The grid lives in a per-CTA global
 // workspace (L2 resident) and is read through L1.
-__global__ void __launch_bounds__(kSweepThreads) k_sweep_generic(SweepDev d)
+// The query's nA x n lookup table is read from shared memory in ANGLE SLICES of slice_rows whole rows
+// (generic_slice_rows).  When the whole table fits (slice_rows >= nA) it is staged once per query and
+// kept across that query's pairs; otherwise every pair stages slice after slice.  The volume is written
+// at sums[p * nA + a] either way and integer sums do not depend on order, so the epilogue is the same.
+__global__ void __launch_bounds__(kSweepThreads) k_sweep_generic(SweepDev d, int slice_rows)
 {
   extern __shared__ __align__(16) unsigned char s_raw[];
-  int32_t * s_off = reinterpret_cast<int32_t *>(s_raw);   // nA * n lookup table of this pair's query
+  int32_t * s_off = reinterpret_cast<int32_t *>(s_raw);   // slice_rows x n lookup rows of this pair's query
   __shared__ double s_dscratch[32];
   __shared__ int s_iscratch[32];
 
@@ -234,6 +238,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_generic(SweepDev d)
   double * probs = d.ws_probs + (size_t)blockIdx.x * d.ws_probs_pitch;
   const int P = d.nX * d.nY, nA = d.nA, n = d.n;
   const int half = d.ksize / 2, taps = d.ksize * d.ksize;
+  const bool whole = slice_rows >= nA;
   int last_q = -1;
 
   for (int pair = blockIdx.x; pair < d.npairs; pair += gridDim.x) {
@@ -245,7 +250,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_generic(SweepDev d)
       for (int i = threadIdx.x; i < n16; i += blockDim.x) g4[i] = make_uint4(0, 0, 0, 0);
       for (int i = n16 * 16 + threadIdx.x; i < d.data_size; i += blockDim.x) grid[i] = 0;
     }
-    if (q != last_q) {
+    if (whole && q != last_q) {
       for (int i = threadIdx.x; i < nA * n; i += blockDim.x) s_off[i] = d.offsets[(size_t)q * nA * n + i];
       last_q = q;
     }
@@ -287,21 +292,29 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_generic(SweepDev d)
       }
     }
     __syncthreads();
-    // (3) correlate: items = (angle, pose), angle-major so a warp shares one lookup row
+    // (3) correlate: items = (angle, pose), angle-major so a warp shares one lookup row; one slice of angles at a time
     const int32_t * pos = d.posidx + (size_t)q * P;
-    for (int item = threadIdx.x; item < nA * P; item += blockDim.x) {
-      const int a = item / P, p = item - a * P;
-      const int base = pos[p];
-      const int32_t * off = s_off + a * n;
-      int acc = 0;
-#pragma unroll 8
-      for (int i = 0; i < n; ++i) {
-        int idx = base + off[i];
-        if ((unsigned)idx < (unsigned)d.data_size) acc += grid[idx];
+    for (int a0 = 0; a0 < nA; a0 += slice_rows) {
+      const int na = min(slice_rows, nA - a0);
+      if (!whole) {
+        const int32_t * src = d.offsets + ((size_t)q * nA + a0) * n;
+        for (int i = threadIdx.x; i < na * n; i += blockDim.x) s_off[i] = src[i];
+        __syncthreads();
       }
-      sums[(size_t)p * nA + a] = acc;
+      for (int item = threadIdx.x; item < na * P; item += blockDim.x) {
+        const int al = item / P, p = item - al * P;
+        const int base = pos[p];
+        const int32_t * off = s_off + al * n;
+        int acc = 0;
+#pragma unroll 8
+        for (int i = 0; i < n; ++i) {
+          int idx = base + off[i];
+          if ((unsigned)idx < (unsigned)d.data_size) acc += grid[idx];
+        }
+        sums[(size_t)p * nA + a0 + al] = acc;
+      }
+      __syncthreads();
     }
-    __syncthreads();
     // (4) reduce
     pair_epilogue(d, pair, q, SumsPoseMajor{sums, nA}, probs, s_dscratch, s_iscratch);
   }
@@ -742,6 +755,16 @@ static void coarse_search(const b200sm * h, double off[2], double res[2])
 
 static bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st);
 
+// shared memory the generic kernel may fill with lookup rows; a query needs at least one row (n <= 51,200 readings)
+constexpr size_t kGenericTableBytes = 200 * 1024;
+// whole angle rows of the lookup table per slice of the generic kernel: all nA when the table fits (one slice, staged once
+// per query), else as many as fit
+static int generic_slice_rows(int nA, int n)
+{
+  const size_t row = (size_t)n * sizeof(int32_t);
+  return (int)std::min<size_t>((size_t)nA, kGenericTableBytes / row);
+}
+
 static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b200_scan * scans, int nscans,
                         const int32_t * chain_start, int nchains, const int32_t * pair_query,
                         const int32_t * pair_chain, int npairs, bool do_penalize)
@@ -826,8 +849,8 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
     S.arena.reserve((size_t)nq * per_query + lists + (size_t)npairs * items * 8);
     S.arena_used = 0;
   }
-  if ((size_t)nA * n * sizeof(int32_t) > 200 * 1024) {
-    set_last_error("sweep: lookup table does not fit shared memory (angle window too wide for the batched path)");
+  if ((size_t)n * sizeof(int32_t) > kGenericTableBytes) {
+    set_last_error("sweep: one lookup row of the query does not fit shared memory (more than 51,200 readings per query)");
     return B200_ERR_UNSUPPORTED;
   }
   S.nq = nq; S.n = n; S.npairs = npairs; S.nscans = nscans; S.do_penalize = do_penalize;
@@ -910,7 +933,7 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   int dev = 0, sms = 132;
   B200_CUDA(cudaGetDevice(&dev));
   B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const size_t smem = (size_t)nA * n * sizeof(int32_t);
+  const size_t smem = (size_t)generic_slice_rows(nA, n) * n * sizeof(int32_t);
   const int per_sm = smem <= 100 * 1024 ? 2 : 1;
   S.blocks = std::min(npairs, sms * per_sm);
   const size_t gpitch = ((size_t)g0.data_size + 255) & ~(size_t)255;
@@ -1162,9 +1185,10 @@ static int sweep_run(b200sm * h)
       k_sweep_fast<<<S.fast_blocks, kFastThreads, S.fast_smem, st>>>(d, S.fast);
       break;
     default: {
-      const size_t smem = (size_t)d.nA * d.n * sizeof(int32_t);
+      const int rows = generic_slice_rows(d.nA, d.n);
+      const size_t smem = (size_t)rows * d.n * sizeof(int32_t);
       B200_CUDA(cudaFuncSetAttribute(k_sweep_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_sweep_generic<<<S.blocks, kSweepThreads, smem, st>>>(d);
+      k_sweep_generic<<<S.blocks, kSweepThreads, smem, st>>>(d, rows);
     }
   }
   B200_CUDA(cudaGetLastError());

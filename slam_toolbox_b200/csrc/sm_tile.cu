@@ -798,6 +798,15 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     S.tile_info[5] = why;
     return false;
   };
+  // Packed fields and their bounds (a refusal runs the sweep on the generic kernel, which takes any n and nA):
+  //   TileSeq.a0 / chunk (int16)   nA <= 4096                                                  -> 2
+  //   item al (6 bits)             nAc <= 63 angles per chunk (the V loop)                     -> 4 when no V fits
+  //   item mpairs (8 bits)         multi entries only in groups of <= kChunkBeams beams: <= 214   (no refusal needed)
+  //   one angle's block            payload <= n + 16 entries, records per the one_angle minimum  -> 8
+  //   TileSeq.nitems (int16)       records of one block                                        -> 10
+  //   item pb / pe (16 bits)       payload entries of one block                                -> 11
+  //   TileSeq.off (int32)          descriptor blob bytes                                       -> 12
+  //   cell-list staging            max_n > 4096: the raster reads the cells from global memory    (no refusal needed)
   if (g.order_dependent) return bail(1);                // AddScan's occupancy test makes the raster sequential (generic kernel)
   if ((g.stride & 1) || nA < 1 || nA > 4096) return bail(2);
   for (int q = 0; q < nq; ++q) {
@@ -1035,9 +1044,10 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
               for (int m = 0; m < 4; ++m) ep += std::max(1, (E.tbl[3 * m + 1] - E.tbl[3 * m] + kChunkBeams - 1) / kChunkBeams);
               const size_t hdr = (((size_t)(npieces + ep) * xtiles * ytiles * 8) + 15) & ~(size_t)15;
               const size_t bytes = (hdr + (pay.size() + E.pay.size()) * 2 + 15) & ~(size_t)15;
-              if (bytes > (size_t)stage_bytes || pay.size() + E.pay.size() > 65535) {   // item ranges are 16-bit
+              const bool wide = pay.size() + E.pay.size() > 65535;   // item records hold 16-bit payload indices (pb, pe)
+              if (bytes > (size_t)stage_bytes || wide) {
                 if (na > 0) break;
-                return bail(8);   // one angle does not fit the staging buffer
+                return bail(wide ? 11 : 8);   // one angle does not fit the 16-bit indices / the staging buffer
               }
               const int shift = (int)pay.size();
               for (int k = 0; k < 12; ++k) tbl.push_back(E.tbl[k] + shift);
@@ -1048,6 +1058,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
             nedge.assign((size_t)na * 4, 0);
             for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)egrp[((size_t)(a + (g2 >> 2)) * nstage + sg) * 4 + (g2 & 3)].size();
             build_block_items(tbl, nedge, na, xtiles, ytiles, items);
+            if (items.size() > 32767) return bail(10);   // TileSeq.nitems is 16-bit
             int32_t * ts = S.tile_stats;
             ts[0] += 1;
             ts[1] += first_sub ? 0 : 1;
@@ -1061,6 +1072,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
             }
             const size_t hdr = ((items.size() * 8) + 15) & ~(size_t)15;
             const size_t bytes = std::max<size_t>(16, (hdr + pay.size() * 2 + 15) & ~(size_t)15);
+            if (blob.size() + bytes > 0x7FFFFFF0u) return bail(12);   // TileSeq.off is a 32-bit byte offset
             TileSeq e{};
             e.off = (int32_t)blob.size();
             e.bytes = (int32_t)bytes;

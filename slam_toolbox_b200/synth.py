@@ -586,6 +586,32 @@ def make_tie_sweep(ks=(1, 2, 23, 24, 25, 100), n_cands: int = 1) -> AdversarialS
     return AdversarialSweep(qr, qp, cr, cp, np.arange(n_cands + 1, dtype=np.int32), (ANGLE_MIN, ANGLE_INC), TIE_CAND_LASER)
 
 
+def highres_laser(n_beams: int, fov_deg: float) -> tuple:
+    """(angle_min, angle_increment) of a laser with n_beams readings centred on the sensor's x axis: fov_deg from the first
+    to the last reading, or, for a full circle (fov_deg >= 360), n_beams readings spaced 360 / n_beams degrees."""
+    fov = math.radians(fov_deg)
+    inc = fov / n_beams if fov_deg >= 360.0 else fov / (n_beams - 1)
+    return -0.5 * fov, inc
+
+
+def make_highres_sweep(n_beams: int, fov_deg: float, *, seed: int = 11, n_queries: int = 1, n_chains: int = 2,
+                       chain_len: int = 1, radius: float = 3.0, inf_frac: float = 0.0) -> AdversarialSweep:
+    """Room scans from one dense laser (highres_laser(n_beams, fov_deg)) for the queries and the candidates: the shape of a
+    0.1 deg lidar (2701 beams over 270 deg, 3600 over 360 deg) or of a 3-D lidar flattened to a scan.  Queries sit in a
+    room of make_world(seed) with make_loop_sweep's drift; candidate chains start within `radius` of the first query."""
+    rng = np.random.default_rng(seed)
+    world = make_world(seed)
+    amin, inc = highres_laser(n_beams, fov_deg)
+    qtrue = np.array([free_pose(world, rng) for _ in range(n_queries)])
+    qr = noisy(raycast(world, qtrue, n_beams=n_beams, angle_min=amin, angle_inc=inc), rng, inf_frac=inf_frac)
+    qpose = qtrue + np.column_stack([rng.normal(0, 0.5, (n_queries, 2)), rng.normal(0, 0.08, n_queries)])
+    starts = poses_near(world, qtrue[0, :2], radius, n_chains, rng)
+    cposes = starts if chain_len == 1 else np.concatenate([chain_poses(world, s, chain_len, rng) for s in starts])
+    cr = noisy(raycast(world, cposes, n_beams=n_beams, angle_min=amin, angle_inc=inc), rng, inf_frac=inf_frac)
+    chain_start = np.arange(0, n_chains * chain_len + 1, chain_len, dtype=np.int32)
+    return AdversarialSweep(qr, qpose, cr, cposes, chain_start, (amin, inc), (amin, inc))
+
+
 def make_long_query_sweep(n: int, seed: int = 7, n_chains: int = 3, inf_frac: float = 0.97) -> AdversarialSweep:
     """One query of n beams over the usual 270 deg field of view (a room scan at n / 1081 times the angular density, a fraction
     inf_frac of the readings replaced by inf) and n_chains room-scan candidates.  With the defaults, n = 10240 and the 4 m /
