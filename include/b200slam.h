@@ -218,13 +218,21 @@ typedef struct b200pg_opts {
   int32_t max_num_consecutive_invalid_steps;  /* 3 (:163)                                       */
   /* linear solver (replaces SPARSE_NORMAL_CHOLESKY, :100-102): block-Jacobi PCG on the
    * normal equations, iterated to ||r|| <= pcg_tolerance * ||b|| */
-  double pcg_tolerance;              /* 1e-9: poses stay within 5e-6 m / 5e-7 rad of the exact-solve LM on cfg4 (1e-8 would not) */
+  double pcg_tolerance;              /* 1e-9: poses stay within 5e-6 m / 5e-7 rad of the exact-solve LM on cfg4 (1e-8 would not);
+                                      * under dogleg the Gauss-Newton solve runs to pcg_tolerance / 10 */
   int32_t pcg_max_iterations;        /* 20000 */
   /* ceres_loss_function (ceres_solver.cpp:82-94): 0 = none (squared loss, the default), 1 = HuberLoss(loss_scale),
    * 2 = CauchyLoss(loss_scale); the reference uses scale 0.7 for both */
   int32_t loss_function;
   double loss_scale;                 /* 0.7 */
+  /* ceres_trust_strategy (ceres_solver.cpp:46-58): 0 = LEVENBERG_MARQUARDT (the default), 1 = DOGLEG.
+   * ceres_dogleg_type (:138-155), read with DOGLEG only: 0 = TRADITIONAL_DOGLEG, 1 = SUBSPACE_DOGLEG.
+   * Other values are refused with B200_ERR_INVALID_ARG. */
+  int32_t trust_region_strategy;
+  int32_t dogleg_type;
 } b200pg_opts;
+/* b200pg_opts and b200pg_summary grew (trust_region_strategy, dogleg_type; linear_solves): the ctypes mirror
+ * (slam_toolbox_b200/api.py PgOpts / PgSummary) and every compiled caller must be rebuilt against this header. */
 
 typedef struct b200pg_summary {
   int32_t iterations;          /* LM iterations (successful + unsuccessful)            */
@@ -240,6 +248,8 @@ typedef struct b200pg_summary {
   int32_t uploaded_edges;      /* constraints copied to the device by this call (the ones added since the last solve) */
   int32_t linear_solver;       /* PCG kernel the plan chose: 0 global block-Jacobi, 1 shared-memory block-Jacobi,
                                 * 3 two-level with 3 coarse modes, 6 two-level with 6 coarse modes; -1 no linear solve planned */
+  int32_t linear_solves;       /* PCG solves this call ran, retries at a larger regulariser included: one per iteration
+                                * under LM; under dogleg none for an iteration that reuses the Gauss-Newton step */
 } b200pg_summary;
 
 typedef struct b200pg b200pg;

@@ -55,7 +55,8 @@ class PgOpts(C.Structure):
                 ("jacobi_scaling", C.c_int32), ("use_nonmonotonic_steps", C.c_int32),
                 ("max_consecutive_nonmonotonic_steps", C.c_int32), ("max_num_consecutive_invalid_steps", C.c_int32),
                 ("pcg_tolerance", C.c_double), ("pcg_max_iterations", C.c_int32),
-                ("loss_function", C.c_int32), ("loss_scale", C.c_double)]
+                ("loss_function", C.c_int32), ("loss_scale", C.c_double),
+                ("trust_region_strategy", C.c_int32), ("dogleg_type", C.c_int32)]
 
 
 class OgParams(C.Structure):
@@ -71,7 +72,8 @@ class PgSummary(C.Structure):
     _fields_ = [("iterations", C.c_int32), ("successful_steps", C.c_int32), ("pcg_iterations", C.c_int32),
                 ("termination", C.c_int32), ("usable", C.c_int32), ("initial_cost", C.c_double), ("final_cost", C.c_double),
                 ("solve_ms", C.c_float), ("kernel_launches", C.c_int64),
-                ("setup_ms", C.c_float), ("wall_ms", C.c_float), ("uploaded_edges", C.c_int32), ("linear_solver", C.c_int32)]
+                ("setup_ms", C.c_float), ("wall_ms", C.c_float), ("uploaded_edges", C.c_int32), ("linear_solver", C.c_int32),
+                ("linear_solves", C.c_int32)]
 
 
 def library_path() -> str:

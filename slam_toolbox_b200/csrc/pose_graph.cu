@@ -23,6 +23,7 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <complex>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
@@ -1168,6 +1169,74 @@ __global__ void __launch_bounds__(kPgThreads) k_pg_model_change(PgDev d)
   if (threadIdx.x == 0) d.partial[blockIdx.x] = s[0];
 }
 
+// ------------------------------------------------------------------------------------------
+// Dogleg (DoglegStrategy, DESIGN.md §4).  In the scaled space of Ceres' dogleg, with D = sqrt(diag):
+//   g_s = g / D,  gn_s = -D y_gn  (y_gn: PCG solution of (H + mu D^2) y = g),  J D^-1 g_s = J~ (g / D^2) = u,
+//   J D^-1 gn_s = -J~ y_gn = -w.
+// The host needs the six Gram scalars of {g_s, gn_s} and of their images {u, -w}; every step the strategy can take
+// is a combination of g_s and gn_s, so the device only ever composes  y = cg (g / D^2) + cy y_gn  (k_pg_dogleg_compose)
+// and k_pg_model_change / k_pg_apply_step run unchanged on it.
+// ------------------------------------------------------------------------------------------
+
+// per node: partials of ||g_s||^2 = sum g^2/D^2, ||gn_s||^2 = sum D^2 y^2, sum g.y (= -g_s.gn_s) -> partial slots 0..2
+__global__ void __launch_bounds__(kPgThreads) k_pg_dogleg_nodes(PgDev d, const double * __restrict__ ygn)
+{
+  __shared__ double red[3 * 32];
+  double s[3] = {0, 0, 0};
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < 3 * d.N; k += gridDim.x * blockDim.x) {
+    const double g = d.g[k], dg = d.diag[k], y = ygn[k];
+    s[0] += g * g / dg;
+    s[1] += dg * y * y;
+    s[2] += g * y;
+  }
+  block_sum<3>(s, red);
+  if (threadIdx.x == 0)
+    for (int k = 0; k < 3; ++k) d.partial[k * kMaxPartials + blockIdx.x] = s[k];
+}
+
+// per edge: u = J~_e (g / D^2), w = J~_e y_gn from the linearisation record; partials of ||u||^2, ||w||^2, u.w -> slots 0..2
+__global__ void __launch_bounds__(kPgThreads) k_pg_dogleg_edges(PgDev d, const double * __restrict__ ygn)
+{
+  __shared__ double red[3 * 32];
+  double s[3] = {0, 0, 0};
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < d.E; e += gridDim.x * blockDim.x) {
+    const int a = d.eidx[2 * e], b = d.eidx[2 * e + 1];
+    const double * L = d.lin + (size_t)kLin * e;
+    double va[3], vb[3], ya[3], yb[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      va[k] = d.g[3 * a + k] / d.diag[3 * a + k]; vb[k] = d.g[3 * b + k] / d.diag[3 * b + k];
+      ya[k] = ygn[3 * a + k]; yb[k] = ygn[3 * b + k];
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      const double * A = L + 3 + 3 * i, * B = L + 12 + 3 * i;
+      const double u = A[0] * va[0] + A[1] * va[1] + A[2] * va[2] + B[0] * vb[0] + B[1] * vb[1] + B[2] * vb[2];
+      const double w = A[0] * ya[0] + A[1] * ya[1] + A[2] * ya[2] + B[0] * yb[0] + B[1] * yb[1] + B[2] * yb[2];
+      s[0] += u * u; s[1] += w * w; s[2] += u * w;
+    }
+  }
+  block_sum<3>(s, red);
+  if (threadIdx.x == 0)
+    for (int k = 0; k < 3; ++k) d.partial[k * kMaxPartials + blockIdx.x] = s[k];
+}
+
+// the dogleg step in the y convention of k_pg_model_change / k_pg_apply_step (step = -y)
+__global__ void k_pg_dogleg_compose(PgDev d, const double * __restrict__ ygn, double cg, double cy)
+{
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < 3 * d.N; k += gridDim.x * blockDim.x)
+    d.y[k] = cg * (d.g[k] / d.diag[k]) + cy * ygn[k];
+}
+
+// fixed-order sums of partial slots 0..n-1 into scalars[slot0 + k] (k_pg_reduce for several sums)
+__global__ void k_pg_reduce_n(PgDev d, int nparts, int n, int slot0)
+{
+  if (threadIdx.x >= n) return;
+  double s = 0;
+  for (int i = 0; i < nparts; ++i) s += d.partial[threadIdx.x * kMaxPartials + i];
+  d.scalars[slot0 + threadIdx.x] = s;
+}
+
 __global__ void k_pg_fill(double * p, double v, int n)
 {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = v;
@@ -1219,6 +1288,7 @@ struct b200pg {
   bool force_global_pcg = false;
   DevBuf<double> d_z, d_U, d_x, d_xc, d_scale, d_lin, d_Hd, d_g, d_diag, d_y, d_pr, d_pz, d_pp0, d_pp1, d_pq, d_Minv,
     d_partial, d_scalars;
+  DevBuf<double> d_ygn;   // dogleg: the Gauss-Newton solution, kept for the iterations that reuse it
   PinBuf<double> h_scalars;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int64_t launches = 0;
@@ -1246,6 +1316,8 @@ void b200pg_defaults(b200pg_opts * o)
   o->pcg_max_iterations = 20000;
   o->loss_function = 0;
   o->loss_scale = 0.7;
+  o->trust_region_strategy = 0;
+  o->dogleg_type = 0;
 }
 
 // karto::Matrix3::Inverse by cofactors (Karto.h:2533-2577) then Eigen's llt().matrixU()
@@ -1300,6 +1372,138 @@ static void grow_keep(DevBuf<T> & b, size_t n, size_t keep, cudaStream_t s)
   std::swap(b.p, nb.p); std::swap(b.cap, nb.cap);
 }
 
+// ---- dogleg strategy: host FP64 algebra on six Gram scalars (DESIGN.md §4) ----
+// Every step the strategy takes is s_s = ca g_s + cb gn_s in the scaled space; the device composes it from (ca, cb).
+constexpr double kDlMinMu = 1e-8, kDlMaxMu = 1.0, kDlMuIncrease = 10.0, kDlKktCosine = 0.99;
+// The Gauss-Newton solve runs 10x tighter than pcg_tolerance: its nearly undamped step (mu ~ 1e-8) carries the PCG error
+// into the iterate in full, and at 1e-9 the final cost of cfg4 (0.05 m / 0.02 rad) is 1.2e-8 away from the exact-solve
+// oracle's, at 1e-10 4.4e-10 (tools/dogleg_study.py on an H100, DESIGN.md §4).
+constexpr double kDlPcgTolFactor = 0.1;
+
+struct DoglegModel {
+  double G[2][2];    // Gram matrix of (g_s, gn_s)
+  double GJ[2][2];   // Gram matrix of their images J D^-1 g_s, J D^-1 gn_s
+  double alpha;      // Cauchy factor ||g_s||^2 / ||J D^-1 g_s||^2
+  bool rank1;
+  double C[2][2];    // orthonormal basis of span{g_s, gn_s}: column k = C[0][k] g_s + C[1][k] gn_s
+  double g2[2], B2[2][2];   // the 2-D model in that basis
+
+  // from k_pg_dogleg_nodes / k_pg_dogleg_edges: sum g^2/D^2, sum D^2 y^2, sum g.y, ||u||^2, ||w||^2, u.w
+  void set(const double * s)
+  {
+    G[0][0] = s[0]; G[1][1] = s[1]; G[0][1] = G[1][0] = -s[2];
+    GJ[0][0] = s[3]; GJ[1][1] = s[4]; GJ[0][1] = GJ[1][0] = -s[5];
+    alpha = G[0][0] / GJ[0][0];
+  }
+  // column-pivoted QR of [g_s gn_s] carried out on the Gram matrix; rank 1 when |R22| <= 2 eps |R11|
+  void subspace()
+  {
+    const int p = G[1][1] > G[0][0] ? 1 : 0, q = 1 - p;
+    const double r11 = sqrt(G[p][p]), r12 = G[p][q] / r11, r22 = sqrt(std::max(0.0, G[q][q] - r12 * r12));
+    rank1 = !(r22 > 2.0 * 2.220446049250313e-16 * r11);
+    C[p][0] = 1.0 / r11; C[q][0] = 0.0;
+    C[p][1] = rank1 ? 0.0 : -r12 / (r11 * r22); C[q][1] = rank1 ? 0.0 : 1.0 / r22;
+    for (int k = 0; k < 2; ++k) g2[k] = C[0][k] * G[0][0] + C[1][k] * G[1][0];
+    for (int k = 0; k < 2; ++k)
+      for (int l = 0; l < 2; ++l) {
+        double s = 0;
+        for (int i = 0; i < 2; ++i)
+          for (int j = 0; j < 2; ++j) s += C[i][k] * GJ[i][j] * C[j][l];
+        B2[k][l] = s;
+      }
+  }
+  double norm(double ca, double cb) const
+  {
+    return sqrt(std::max(0.0, ca * ca * G[0][0] + 2.0 * ca * cb * G[0][1] + cb * cb * G[1][1]));
+  }
+};
+
+// the four complex roots of c[0] y^4 + ... + c[4] (Aberth-Ehrlich iteration; no LAPACK in this library)
+static void quartic_roots(const double c[5], std::complex<double> z[4])
+{
+  using cd = std::complex<double>;
+  double a[5], rad = 0.0;
+  for (int k = 0; k < 5; ++k) a[k] = c[k] / c[0];
+  for (int k = 1; k < 5; ++k) rad = std::max(rad, pow(fabs(a[k]), 1.0 / k));
+  if (!(rad > 0.0)) rad = 1.0;
+  for (int k = 0; k < 4; ++k) z[k] = std::polar(rad, 0.7 + 2.0 * M_PI * k / 4.0);
+  for (int iter = 0; iter < 500; ++iter) {
+    bool moved = false;
+    for (int i = 0; i < 4; ++i) {
+      cd p = a[0], dp = 0.0;
+      for (int k = 1; k < 5; ++k) { dp = dp * z[i] + p; p = p * z[i] + a[k]; }
+      if (p == 0.0) continue;
+      cd s = 0.0;
+      for (int j = 0; j < 4; ++j)
+        if (j != i) s += 1.0 / (z[i] - z[j]);
+      const cd ratio = p / dp, w = ratio / (1.0 - ratio * s);
+      if (!std::isfinite(w.real()) || !std::isfinite(w.imag())) continue;
+      if (std::abs(w) > 1e-16 * std::abs(z[i])) moved = true;
+      z[i] -= w;
+    }
+    if (!moved) break;
+  }
+}
+
+// minimum of 1/2 x^T B x + g^T x on ||x|| = r over the stationary points (B + y I) x = -g, y a root of the quartic;
+// false when no root gives a usable point or the first-order (KKT) check fails
+static bool boundary_minimum(const double g[2], const double B[2][2], double r, double x[2])
+{
+  const double tr = B[0][0] + B[1][1], det = B[0][0] * B[1][1] - B[0][1] * B[1][0];
+  const double ag0 = B[1][1] * g[0] - B[0][1] * g[1], ag1 = -B[1][0] * g[0] + B[0][0] * g[1];
+  const double r2 = r * r;
+  const double poly[5] = {r2, 2.0 * r2 * tr, r2 * (tr * tr + 2.0 * det) - (g[0] * g[0] + g[1] * g[1]),
+                          -2.0 * ((g[0] * ag0 + g[1] * ag1) - r2 * det * tr), r2 * det * det - (ag0 * ag0 + ag1 * ag1)};
+  std::complex<double> z[4];
+  quartic_roots(poly, z);
+  bool found = false;
+  double best_f = INFINITY;
+  for (int k = 0; k < 4; ++k) {
+    const double y = z[k].real();
+    const double m00 = B[0][0] + y, m01 = B[0][1], m10 = B[1][0], m11 = B[1][1] + y;
+    const double dm = m00 * m11 - m01 * m10;
+    if (dm == 0.0) continue;
+    double x0 = -(m11 * g[0] - m01 * g[1]) / dm, x1 = -(-m10 * g[0] + m00 * g[1]) / dm;
+    const double n = sqrt(x0 * x0 + x1 * x1);
+    if (!std::isfinite(n) || !(n > 0.0)) continue;
+    x0 *= r / n; x1 *= r / n;
+    const double f = 0.5 * (x0 * (B[0][0] * x0 + B[0][1] * x1) + x1 * (B[1][0] * x0 + B[1][1] * x1)) + g[0] * x0 + g[1] * x1;
+    if (f < best_f) { best_f = f; x[0] = x0; x[1] = x1; found = true; }
+  }
+  if (!found) return false;
+  const double q0 = B[0][0] * x[0] + B[0][1] * x[1] + g[0], q1 = B[1][0] * x[0] + B[1][1] * x[1] + g[1];
+  const double cosine = -(x[0] * q0 + x[1] * q1) / (sqrt(x[0] * x[0] + x[1] * x[1]) * sqrt(q0 * q0 + q1 * q1));
+  return !(cosine < kDlKktCosine);
+}
+
+// ComputeTraditionalDoglegStep / ComputeSubspaceDoglegStep: coefficients of s_s = ca g_s + cb gn_s and ||s_s||
+static void traditional_step(const DoglegModel & m, double radius, double & ca, double & cb, double & step_norm)
+{
+  const double gn_norm = sqrt(m.G[1][1]), g_norm = sqrt(m.G[0][0]);
+  if (gn_norm <= radius) { ca = 0.0; cb = 1.0; step_norm = gn_norm; return; }
+  if (m.alpha * g_norm >= radius) { ca = -radius / g_norm; cb = 0.0; step_norm = radius; return; }
+  // the point where the segment a = -alpha g_s -> b = gn_s crosses ||.|| = radius, in Ceres' cancellation-safe form
+  const double b_dot_a = -m.alpha * m.G[0][1], a_sq = m.alpha * m.alpha * m.G[0][0];
+  const double bma_sq = a_sq - 2.0 * b_dot_a + m.G[1][1];
+  const double c = b_dot_a - a_sq;
+  const double dd = sqrt(c * c + bma_sq * (radius * radius - a_sq));
+  const double beta = c <= 0 ? (dd - c) / bma_sq : (radius * radius - a_sq) / (dd + c);
+  ca = -(1.0 - beta) * m.alpha; cb = beta;
+  step_norm = m.norm(ca, cb);
+}
+
+static void subspace_step(const DoglegModel & m, double radius, double & ca, double & cb, double & step_norm)
+{
+  const double gn_norm = sqrt(m.G[1][1]);
+  if (gn_norm <= radius) { ca = 0.0; cb = 1.0; step_norm = gn_norm; return; }
+  if (m.rank1) { ca = -radius / sqrt(m.G[0][0]); cb = 0.0; step_norm = radius; return; }
+  double x[2];
+  if (!boundary_minimum(m.g2, m.B2, radius, x)) { traditional_step(m, radius, ca, cb, step_norm); return; }
+  ca = m.C[0][0] * x[0] + m.C[0][1] * x[1];
+  cb = m.C[1][0] * x[0] + m.C[1][1] * x[1];
+  step_norm = radius;
+}
+
 struct Lm {
   b200pg * h;
   PgDev d;
@@ -1321,10 +1525,27 @@ struct Lm {
     B200_CUDA(cudaStreamSynchronize(st));
     return h->h_scalars.p[slot];
   }
-  void fetch()
+  void fetch(int n = 16)
   {
-    B200_CUDA(cudaMemcpyAsync(h->h_scalars.p, h->d_scalars.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaMemcpyAsync(h->h_scalars.p, h->d_scalars.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
+  }
+  // one PCG solve of (H + shift * diag) y = g on the planned kernel; scalars[8] = iterations, [9] = relative residual
+  void pcg(double shift, double tol, int max_iter)
+  {
+    if (use_2lvl) {
+      B200_CUDA(cudaMemsetAsync(h->d_bar.p, 0, (size_t)(blocks2 + 1) * sizeof(unsigned int), st));
+      void * args[] = {&d, &cfg2, &shift, &tol, &max_iter};
+      B200_CUDA(cudaLaunchCooperativeKernel(cm2 == 6 ? (void *)k_pg_pcg_2lvl<6> : (void *)k_pg_pcg_2lvl<3>, dim3(blocks2), dim3(256), args, smem2_bytes, st));
+    } else if (use_smem) {
+      B200_CUDA(cudaMemsetAsync(h->d_bar.p, 0, sizeof(unsigned int), st));
+      void * args[] = {&d, &cfg, &shift, &tol, &max_iter};
+      B200_CUDA(cudaLaunchCooperativeKernel((void *)k_pg_pcg_smem, dim3(smem_blocks), dim3(512), args, smem_bytes, st));
+    } else {
+      void * args[] = {&d, &shift, &tol, &max_iter};
+      B200_CUDA(cudaLaunchCooperativeKernel((void *)k_pg_pcg, dim3(pcg_blocks), dim3(kPgThreads), args, 0, st));
+    }
+    h->launches++;
   }
   void launched() { B200_CUDA(cudaGetLastError()); h->launches++; }
 
@@ -1428,7 +1649,10 @@ static int solve(b200pg * h, b200pg_summary * sum)
   h->d_xc.reserve(n3); h->d_scale.reserve(n3); h->d_lin.reserve((size_t)kLin * E); h->d_Hd.reserve(6 * (size_t)N);
   h->d_g.reserve(n3); h->d_diag.reserve(n3); h->d_y.reserve(n3); h->d_pr.reserve(n3); h->d_pz.reserve(n3);
   h->d_pp0.reserve(n3); h->d_pp1.reserve(n3); h->d_pq.reserve(n3); h->d_Minv.reserve(6 * (size_t)N);
-  h->d_partial.reserve((size_t)kMaxPartials * 8); h->d_scalars.reserve(16); h->h_scalars.reserve(16);
+  h->d_partial.reserve((size_t)kMaxPartials * 8); h->d_scalars.reserve(32); h->h_scalars.reserve(32);
+  const bool dogleg = o.trust_region_strategy == 1, subspace = o.dogleg_type == 1;
+  const double gn_tol = kDlPcgTolFactor * o.pcg_tolerance;   // dogleg's Gauss-Newton solve (DESIGN.md §4)
+  if (dogleg) h->d_ygn.reserve(n3);
 
   Lm L;
   L.h = h; L.st = st;
@@ -1543,6 +1767,10 @@ static int solve(b200pg * h, b200pg_summary * sum)
 
   double radius = o.initial_trust_region_radius, decrease_factor = 2.0;
   bool reuse_diagonal = false;
+  // DoglegStrategy state: regulariser mu, reuse of the last Gauss-Newton step, its model, norm of the last step taken
+  double mu = kDlMinMu, dl_step_norm = 0.0;
+  bool dl_reuse = false;
+  DoglegModel dm{};
   const int max_nonmono = o.use_nonmonotonic_steps ? o.max_consecutive_nonmonotonic_steps : 0;
   double ev_min = cost, ev_cur = cost, ev_ref = cost, ev_cand = cost, acc_ref = 0.0, acc_cand = 0.0;
   int n_nonmono = 0, invalid_steps = 0, it = 0;
@@ -1557,28 +1785,51 @@ static int solve(b200pg * h, b200pg_summary * sum)
     if (step_successful && gmax <= o.gradient_tolerance) { S.termination = 1; break; }
     if (radius <= o.min_trust_region_radius) { S.termination = 4; break; }
     ++it;
-    NvtxRange nvtx_it("b200pg LM iteration");
+    NvtxRange nvtx_it(dogleg ? "b200pg dogleg iteration" : "b200pg LM iteration");
     step_successful = false;
-    // LevenbergMarquardtStrategy::ComputeStep
-    if (!reuse_diagonal) { k_pg_diag<<<L.blocksN, kPgThreads, 0, st>>>(d, o.min_lm_diagonal, o.max_lm_diagonal); L.launched(); }
-    {
-      double inv_radius = 1.0 / radius, tol = o.pcg_tolerance;
-      int max_iter = o.pcg_max_iterations;
-      if (L.use_2lvl) {
-        B200_CUDA(cudaMemsetAsync(h->d_bar.p, 0, (size_t)(L.blocks2 + 1) * sizeof(unsigned int), st));
-        void * args[] = {&d, &L.cfg2, &inv_radius, &tol, &max_iter};
-        B200_CUDA(cudaLaunchCooperativeKernel(L.cm2 == 6 ? (void *)k_pg_pcg_2lvl<6> : (void *)k_pg_pcg_2lvl<3>, dim3(L.blocks2), dim3(256), args, L.smem2_bytes, st));
-      } else if (L.use_smem) {
-        B200_CUDA(cudaMemsetAsync(h->d_bar.p, 0, sizeof(unsigned int), st));
-        void * args[] = {&d, &L.cfg, &inv_radius, &tol, &max_iter};
-        B200_CUDA(cudaLaunchCooperativeKernel((void *)k_pg_pcg_smem, dim3(L.smem_blocks), dim3(512), args, L.smem_bytes, st));
-      } else {
-        void * args[] = {&d, &inv_radius, &tol, &max_iter};
-        B200_CUDA(cudaLaunchCooperativeKernel((void *)k_pg_pcg, dim3(L.pcg_blocks), dim3(kPgThreads), args, 0, st));
+    if (dogleg) {
+      // DoglegStrategy::ComputeStep
+      bool solved = true;
+      if (!dl_reuse) {
+        k_pg_diag<<<L.blocksN, kPgThreads, 0, st>>>(d, o.min_lm_diagonal, o.max_lm_diagonal); L.launched();
+        solved = false;
+        while (mu < kDlMaxMu) {   // Gauss-Newton step: (H + mu D^2) y = g, mu grows while the solve fails
+          L.pcg(mu, gn_tol, o.pcg_max_iterations);
+          S.linear_solves++;
+          B200_CUDA(cudaMemcpyAsync(h->d_ygn.p, d.y, n3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+          k_pg_dogleg_nodes<<<L.blocksN, kPgThreads, 0, st>>>(d, h->d_ygn.p); L.launched();
+          k_pg_reduce_n<<<1, 32, 0, st>>>(d, L.blocksN, 3, 16); L.launched();
+          k_pg_dogleg_edges<<<L.blocksE, kPgThreads, 0, st>>>(d, h->d_ygn.p); L.launched();
+          k_pg_reduce_n<<<1, 32, 0, st>>>(d, L.blocksE, 3, 19); L.launched();
+          L.fetch(22);
+          const double * sc = h->h_scalars.p;
+          S.pcg_iterations += (int)sc[8];
+          solved = sc[9] <= gn_tol;
+          for (int k = 16; k < 22; ++k) solved = solved && std::isfinite(sc[k]);
+          if (solved) { dm.set(sc + 16); break; }
+          mu *= kDlMuIncrease;
+        }
+        if (solved) {
+          if (subspace) dm.subspace();
+          dl_reuse = true;
+        }
       }
-      h->launches++;
+      if (!solved) {   // linear solver failure: an invalid step (DoglegStrategy::StepIsInvalid)
+        if (++invalid_steps >= o.max_num_consecutive_invalid_steps) { S.termination = 5; S.usable = 0; break; }
+        mu *= kDlMuIncrease; dl_reuse = false;
+        continue;
+      }
+      double ca, cb;
+      if (subspace) subspace_step(dm, radius, ca, cb, dl_step_norm);
+      else traditional_step(dm, radius, ca, cb, dl_step_norm);
+      k_pg_dogleg_compose<<<L.blocksN, kPgThreads, 0, st>>>(d, h->d_ygn.p, -ca, cb); L.launched();
+    } else {
+      // LevenbergMarquardtStrategy::ComputeStep
+      if (!reuse_diagonal) { k_pg_diag<<<L.blocksN, kPgThreads, 0, st>>>(d, o.min_lm_diagonal, o.max_lm_diagonal); L.launched(); }
+      L.pcg(1.0 / radius, o.pcg_tolerance, o.pcg_max_iterations);
+      S.linear_solves++;
+      reuse_diagonal = true;
     }
-    reuse_diagonal = true;
     k_pg_model_change<<<L.blocksE, kPgThreads, 0, st>>>(d); L.launched();
     k_pg_reduce<<<1, 32, 0, st>>>(d, L.blocksE, 4, -1); L.launched();
     k_pg_apply_step<<<L.blocksN, kPgThreads, 0, st>>>(d); L.launched();
@@ -1586,8 +1837,8 @@ static int solve(b200pg * h, b200pg_summary * sum)
     L.linearize(1, 1);   // scalars[1] = cost(xc)
     L.fetch();
     const double * sc = h->h_scalars.p;
-    S.pcg_iterations += (int)sc[8];
-    if (h->debug && L.use_2lvl)
+    if (!dogleg) S.pcg_iterations += (int)sc[8];   // dogleg counted its solves above
+    if (h->debug && L.use_2lvl && !dogleg)
       fprintf(stderr, "[b200pg] lm %d: pcg %d it, setup %.1f us, gauss-jordan %.1f us, cg %.1f us (%.2f us/it: gather %.2f spmv+reduce %.2f exch1 %.2f precond %.2f exch2 %.2f)\n", it, (int)sc[8],
               sc[10] * 1e-3, sc[11] * 1e-3, sc[12] * 1e-3, sc[12] * 1e-3 / std::max(1.0, sc[8]), sc[13] * 1e-3 / std::max(1.0, sc[8]),
               sc[14] * 1e-3 / std::max(1.0, sc[8]), sc[15] * 1e-3 / std::max(1.0, sc[8]), sc[6] * 1e-3 / std::max(1.0, sc[8]), sc[7] * 1e-3 / std::max(1.0, sc[8]));
@@ -1596,7 +1847,8 @@ static int solve(b200pg * h, b200pg_summary * sum)
     const bool valid = finite && model_cost_change > 0.0;
     if (!valid) {   // HandleInvalidStep
       if (++invalid_steps >= o.max_num_consecutive_invalid_steps) { S.termination = 5; S.usable = 0; break; }
-      radius /= decrease_factor; decrease_factor *= 2.0;
+      if (dogleg) { mu *= kDlMuIncrease; dl_reuse = false; }   // DoglegStrategy::StepIsInvalid: radius unchanged
+      else { radius /= decrease_factor; decrease_factor *= 2.0; }
       continue;
     }
     invalid_steps = 0;
@@ -1615,8 +1867,15 @@ static int solve(b200pg * h, b200pg_summary * sum)
       gmax = h->h_scalars.p[2]; x_norm = sqrt(h->h_scalars.p[3]);
       step_successful = true;
       S.successful_steps++;
-      radius = std::min(o.max_trust_region_radius, radius / std::max(1.0 / 3.0, 1.0 - pow(2.0 * quality - 1.0, 3)));
-      decrease_factor = 2.0; reuse_diagonal = false;
+      if (dogleg) {   // DoglegStrategy::StepAccepted (no clamp to max_trust_region_radius, DESIGN.md §4)
+        if (quality < 0.25) radius *= 0.5;
+        if (quality > 0.75) radius = std::max(radius, 3.0 * dl_step_norm);
+        mu = std::max(kDlMinMu, mu / 5.0);
+        dl_reuse = false;
+      } else {
+        radius = std::min(o.max_trust_region_radius, radius / std::max(1.0 / 3.0, 1.0 - pow(2.0 * quality - 1.0, 3)));
+        decrease_factor = 2.0; reuse_diagonal = false;
+      }
       ev_cur = cost; acc_cand += model_cost_change; acc_ref += model_cost_change;
       if (ev_cur < ev_min) { ev_min = ev_cur; n_nonmono = 0; ev_cand = ev_cur; acc_cand = 0.0; }
       else { ++n_nonmono; if (ev_cur > ev_cand) { ev_cand = ev_cur; acc_cand = 0.0; } }
@@ -1632,6 +1891,8 @@ static int solve(b200pg * h, b200pg_summary * sum)
         B200_CUDA(cudaStreamSynchronize(st));
         have_best_on_device_x = false;
       }
+    } else if (dogleg) {   // DoglegStrategy::StepRejected: shrink the region, keep the Gauss-Newton step
+      radius *= 0.5; dl_reuse = true;
     } else {   // HandleUnsuccessfulStep
       radius /= decrease_factor; decrease_factor *= 2.0; reuse_diagonal = true;
     }
@@ -1681,7 +1942,8 @@ int b200pg_create(const b200pg_opts * opts, b200pg ** out)
   if (opts) h->o = *opts; else b200pg_defaults(&h->o);
   if (h->o.max_num_iterations < 0 || !(h->o.pcg_tolerance > 0) || h->o.pcg_max_iterations <= 0 ||
       !(h->o.initial_trust_region_radius > 0) || h->o.loss_function < 0 || h->o.loss_function > 2 ||
-      (h->o.loss_function != 0 && !(h->o.loss_scale > 0))) {
+      (h->o.loss_function != 0 && !(h->o.loss_scale > 0)) || h->o.trust_region_strategy < 0 || h->o.trust_region_strategy > 1 ||
+      h->o.dogleg_type < 0 || h->o.dogleg_type > 1) {
     set_last_error("b200pg_create: invalid options");
     return B200_ERR_INVALID_ARG;
   }
@@ -1708,7 +1970,8 @@ void b200pg_destroy(b200pg * h)
 static bool valid_opts(const b200pg_opts & o)
 {
   return !(o.max_num_iterations < 0 || !(o.pcg_tolerance > 0) || o.pcg_max_iterations <= 0 || !(o.initial_trust_region_radius > 0) ||
-           o.loss_function < 0 || o.loss_function > 2 || (o.loss_function != 0 && !(o.loss_scale > 0)));
+           o.loss_function < 0 || o.loss_function > 2 || (o.loss_function != 0 && !(o.loss_scale > 0)) ||
+           o.trust_region_strategy < 0 || o.trust_region_strategy > 1 || o.dogleg_type < 0 || o.dogleg_type > 1);
 }
 
 int b200pg_set_opts(b200pg * h, const b200pg_opts * opts)
