@@ -90,7 +90,12 @@ int b200sm_set_stream(b200sm * h, void * cuda_stream);
 
 /* ScanMatcher::MatchScan(pScan, rBaseScans, rMean, rCovariance, doPenalize, doRefineMatch)
  * (Mapper.cpp:534-639).  base[0..nbase) in the order of the reference's scan vector / map
- * (order is part of the contract: SURVEY.md 7, hard part 2).  cov is row-major 3x3. */
+ * (order is part of the contract: SURVEY.md 7, hard part 2).  cov is row-major 3x3.
+ * Bounds (this call and b200sm_correlate): a query of at most 51,200 readings (one lookup row of
+ * n int32 must fit 200 KB of shared memory; more -> B200_ERR_UNSUPPORTED once the raster is built,
+ * before any correlation kernel runs); at most 2^26 poses (nX * nY * nAngles) per pass, split
+ * between positions and angles in any way (B200_ERR_INVALID_ARG above that); a correlation ROI narrower than 32,768 cells
+ * (b200sm_create returns B200_ERR_UNSUPPORTED otherwise). */
 int b200sm_match(b200sm * h, const b200_scan * query, const b200_scan * base, int32_t nbase,
                  int32_t do_penalize, int32_t do_refine, double mean[3], double cov[9],
                  double * response);

@@ -199,33 +199,39 @@ __global__ void k_stamp(uint8_t * __restrict__ grid, int stride, int roi_x, int 
 // lanes -- consecutive poses are 2 cells apart, so one warp load touches 1-2 sectors per grid row) and splits the beams over
 // its kCorrWarps warps (interleaved), each lane keeping 8 loads in flight; the partial sums meet in shared memory.
 // Round 1's kernel ran one thread per pose over all 1081 beams, at low occupancy and few loads in flight.
+// gridDim.y is capped at 65,535 (kMaxGridY) while a window may have more angles (+-180 deg at 0.005 deg: 72,001): a block then
+// takes angles blockIdx.y, blockIdx.y + gridDim.y, ...
 constexpr int kCorrWarps = 8;
+constexpr int kMaxGridY = 65535;
 __global__ void __launch_bounds__(32 * kCorrWarps) k_correlate(const uint8_t * __restrict__ grid, int data_size,
                                                                const int32_t * __restrict__ offsets, const int32_t * __restrict__ pos,
                                                                int P, int nA, int n, int32_t * __restrict__ sums)
 {
   extern __shared__ int32_t s_off[];
   __shared__ int s_part[kCorrWarps][32];
-  const int a = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) s_off[i] = offsets[(size_t)a * n + i];
-  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int p = blockIdx.x * 32 + lane;
-  int acc = 0;
-  if (p < P) {
-    const int base = pos[p];
+  const int base = p < P ? pos[p] : 0;
+  for (int a = blockIdx.y; a < nA; a += gridDim.y) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) s_off[i] = offsets[(size_t)a * n + i];
+    __syncthreads();
+    int acc = 0;
+    if (p < P) {
 #pragma unroll 8
-    for (int i = warp; i < n; i += kCorrWarps) {
-      const int idx = base + s_off[i];
-      if ((unsigned)idx < (unsigned)data_size) acc += __ldg(grid + idx);
+      for (int i = warp; i < n; i += kCorrWarps) {
+        const int idx = base + s_off[i];
+        if ((unsigned)idx < (unsigned)data_size) acc += __ldg(grid + idx);
+      }
     }
-  }
-  s_part[warp][lane] = acc;
-  __syncthreads();
-  if (warp == 0 && p < P) {
-    int t = 0;
+    s_part[warp][lane] = acc;
+    __syncthreads();
+    if (warp == 0 && p < P) {
+      int t = 0;
 #pragma unroll
-    for (int w = 0; w < kCorrWarps; ++w) t += s_part[w][lane];
-    sums[(size_t)p * nA + a] = t;
+      for (int w = 0; w < kCorrWarps; ++w) t += s_part[w][lane];
+      sums[(size_t)p * nA + a] = t;
+    }
+    if (a + gridDim.y < nA) __syncthreads();   // every warp is done with this angle's s_off and s_part before the next is staged
   }
 }
 
@@ -706,7 +712,7 @@ static const int32_t * device_volume(b200sm * h, const CorrPlan & pl)
     k_correlate_few<<<(items + 7) / 8, 256, 0, h->stream>>>(h->d_grid.p, g.data_size, h->d_offsets.p, h->d_offsets.p + noff, P, pl.nA,
                                                            pl.n, h->d_sums.p);
   } else {
-    dim3 grid((P + 31) / 32, pl.nA);
+    dim3 grid((P + 31) / 32, std::min(pl.nA, kMaxGridY));
     size_t smem = (size_t)pl.n * sizeof(int32_t);
     if (smem > 40 * 1024) B200_CUDA(cudaFuncSetAttribute(k_correlate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_correlate<<<grid, 32 * kCorrWarps, smem, h->stream>>>(h->d_grid.p, g.data_size, h->d_offsets.p, h->d_offsets.p + noff, P,

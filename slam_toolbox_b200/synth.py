@@ -623,3 +623,126 @@ def make_long_query_sweep(n: int, seed: int = 7, n_chains: int = 3, inf_frac: fl
     qr = noisy(raycast(ls.world, ls.query_true, n_beams=n, angle_inc=inc), rng)
     qr[:, rng.random(n) < inf_frac] = np.inf
     return AdversarialSweep(qr, ls.query_poses, ls.cand_ranges, ls.cand_poses, ls.chain_start, (ANGLE_MIN, inc), (ANGLE_MIN, ANGLE_INC))
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Single-match inputs (one query against a running buffer of base scans) at the poses, beam counts and rasters the sequential
+# cases never produce.  A base scan given as points carries them directly (ranges = distances from its pose), so a test can build
+# rasters no laser draws.
+# ---------------------------------------------------------------------------------------------------------------------------
+@dataclass
+class SingleMatchCase:
+    query_ranges: np.ndarray          # (n,)
+    query_pose: np.ndarray            # (3,)  reported sensor pose
+    base_ranges: np.ndarray           # (B, m)
+    base_poses: np.ndarray            # (B, 3)
+    query_laser: tuple = (ANGLE_MIN, ANGLE_INC)
+    base_laser: tuple = (ANGLE_MIN, ANGLE_INC)
+
+
+def _move_scene(poses: np.ndarray, src: np.ndarray, dst: np.ndarray) -> np.ndarray:
+    """poses (N,3) under the rigid motion that takes pose src to pose dst (headings are not wrapped)"""
+    c, s = math.cos(dst[2] - src[2]), math.sin(dst[2] - src[2])
+    dx, dy = poses[:, 0] - src[0], poses[:, 1] - src[1]
+    return np.column_stack([dst[0] + c * dx - s * dy, dst[1] + s * dx + c * dy, poses[:, 2] + (dst[2] - src[2])])
+
+
+def make_single_match_case(seed: int, *, query: str = "match", search_size: float = 1.0, buffer_len: int = 6,
+                           n_beams: int = N_BEAMS, fov_deg: float = 270.0, pose=None, inf_frac: float = 0.02) -> SingleMatchCase:
+    """One query against a chain of buffer_len room scans (the standard laser) spaced 0.5 m, ending at the query's true pose.
+
+    query      'match'    reported pose = true pose + odometry noise
+               'partial'  reported 0.75 * search_size off in x (beyond the search window's half width) and 0.05 rad off: only
+                          part of the scan lines up anywhere in the window
+               'far'      all but the shortest tenth of the readings dropped (inf), reported left of every base point by more
+                          than those readings, the search window and the smear can bridge: the best response is zero, but the correlation grid (centred on the
+                          reported pose, range threshold >= 6 m) still holds base points
+    n_beams, fov_deg   the query's laser (highres_laser); the base scans keep the standard laser
+    pose       if given, the whole scene is moved rigidly so that the reported query pose is exactly `pose` (the origin, a
+               heading near +-pi or beyond 2 pi, large world coordinates)"""
+    rng = np.random.default_rng(seed)
+    world = make_world(seed)
+    traj = chain_poses(world, free_pose(world, rng), buffer_len + 1, rng)
+    qtrue = traj[-1]
+    base_ranges = noisy(raycast(world, traj[:-1]), rng, inf_frac=inf_frac)
+    amin, inc = highres_laser(n_beams, fov_deg) if n_beams != N_BEAMS else (ANGLE_MIN, ANGLE_INC)
+    qr = noisy(raycast(world, qtrue, n_beams=n_beams, angle_min=amin, angle_inc=inc), rng, inf_frac=inf_frac)[0]
+    reported = qtrue + np.array([rng.normal(0, 0.03), rng.normal(0, 0.03), rng.normal(0, 0.01)])
+    if query == "partial":
+        reported = qtrue + np.array([0.75 * search_size, 0.0, 0.05])
+    elif query == "far":
+        short_range = np.sort(qr[np.isfinite(qr)])[np.isfinite(qr).sum() // 10]
+        qr = np.where(qr > short_range, np.inf, qr)
+        ang = traj[:-1, 2:3] + ANGLE_MIN + np.arange(N_BEAMS) * ANGLE_INC
+        px = np.where(np.isfinite(base_ranges), traj[:-1, 0:1] + base_ranges * np.cos(ang), np.inf)
+        reported = np.array([px.min() - (short_range + 0.75 * search_size + 1.5), qtrue[1], qtrue[2]])
+    elif query != "match":
+        raise ValueError(f"unknown query kind {query!r}")
+    base_poses = traj[:-1]
+    if pose is not None:
+        pose = np.asarray(pose, dtype=np.float64)
+        base_poses = _move_scene(base_poses, reported, pose)
+        reported = pose.copy()
+    return SingleMatchCase(qr, reported, base_ranges, base_poses, (amin, inc), (ANGLE_MIN, ANGLE_INC))
+
+
+def make_few_beam_query(case: SingleMatchCase, n_readings: int) -> SingleMatchCase:
+    """The case's query with all but n_readings evenly spread readings replaced by inf"""
+    keep = np.linspace(0, len(case.query_ranges) - 1, n_readings).astype(int)
+    qr = np.full_like(case.query_ranges, np.inf)
+    qr[keep] = case.query_ranges[keep]
+    return SingleMatchCase(qr, case.query_pose, case.base_ranges, case.base_poses, case.query_laser, case.base_laser)
+
+
+def half_cell_centres(offset: float, resolution: float, cells, ulps: int = 2) -> np.ndarray:
+    """Coordinates offset + (k + 0.5) * resolution for every k in cells, each also moved by 1..ulps units in the last place either
+    way: the centres where a fine search's cell map rounds in both directions"""
+    scale = 1.0 / resolution
+    out = []
+    for k in cells:
+        c = offset + (k + 0.5) / scale
+        for d in range(-ulps, ulps + 1):
+            x = c
+            for _ in range(abs(d)):
+                x = float(np.nextafter(x, np.inf if d > 0 else -np.inf))
+            out.append(x)
+    return np.array(out)
+
+
+def points_scan(points: np.ndarray, pose) -> tuple:
+    """(ranges, points, pose) of a base scan given by its points"""
+    pts = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 2)
+    pose = np.asarray(pose, dtype=np.float64)
+    return np.hypot(pts[:, 0] - pose[0], pts[:, 1] - pose[1]), pts, pose
+
+
+def make_dense_base(center, resolution: float, n_clusters: int = 12, per_cluster: int = 300, radius: float = 1.2,
+                    seed: int = 5) -> list:
+    """One base scan whose points pile up in few cells: n_clusters clusters of per_cluster points, each within a tenth of a cell,
+    on a circle of `radius` around `center` (a sensor there), visited counter-clockwise so that FindValidPoints keeps every
+    cluster but the last"""
+    rng = np.random.default_rng(seed)
+    c = np.asarray(center, dtype=np.float64)
+    pts = []
+    for k in range(n_clusters):
+        a = 2 * math.pi * k / n_clusters
+        p = c[:2] + radius * np.array([math.cos(a), math.sin(a)])
+        pts.append(p + rng.uniform(-0.05 * resolution, 0.05 * resolution, (per_cluster, 2)))
+    return [points_scan(np.concatenate(pts), c)]
+
+
+def make_roi_edge_base(query_pose, resolution: float, roi_w: int) -> list:
+    """Base scans on the border of the correlation grid's region of interest around query_pose (roi_w cells wide, the grid
+    offset of ScanMatcher::MatchScan, Mapper.cpp:560-569): one scan along the first and last ROI rows and columns, one along
+    the cells just outside them, both counter-clockwise around the query"""
+    q = np.asarray(query_pose, dtype=np.float64)
+    res = 1.0 / (1.0 / resolution)
+    off = q[:2] - 0.5 * (roi_w - 1) * res
+    out = []
+    for lo, hi in ((0, roi_w - 1), (-1, roi_w)):
+        k = np.arange(lo, hi)
+        ring = np.concatenate([np.column_stack([k, np.full_like(k, lo)]), np.column_stack([np.full_like(k, hi), k]),
+                               np.column_stack([hi - (k - lo), np.full_like(k, hi)]),
+                               np.column_stack([np.full_like(k, lo), hi - (k - lo)])])
+        out.append(points_scan(off[None, :] + ring * res, q))
+    return out
