@@ -746,3 +746,98 @@ def make_roi_edge_base(query_pose, resolution: float, roi_w: int) -> list:
                                np.column_stack([np.full_like(k, lo), hi - (k - lo)])])
         out.append(points_scan(off[None, :] + ring * res, q))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Crafted occupancy-grid inputs: readings along exact axes, at half cells and where a fused multiply-add would round the
+# clipped end of an over-range beam into another cell.  LocalizedRangeScan::Update computes a beam's angle as
+# (heading + angle_min) + k * angle_increment; a heading can make that exactly 0, +-pi/2 (as doubles) or pi for many beams k.
+# cos(0) = 1, sin(0) = 0 and cos(pi) = -1 in double, so such a beam's point is (x + r, y), (x - r, ~y); at +-pi/2 the y
+# coordinate is y +- r.  Scans are the standard laser with every other reading inf.
+# ---------------------------------------------------------------------------------------------------------------------------
+AXIS_ANGLES = {"+x": 0.0, "+y": math.pi / 2, "-y": -math.pi / 2, "-x": math.pi}
+
+
+def _ulp_steps(x: float, n: int):
+    """x moved by -n..n units in the last place"""
+    out = [x]
+    lo = hi = x
+    for _ in range(n):
+        lo, hi = float(np.nextafter(lo, -np.inf)), float(np.nextafter(hi, np.inf))
+        out += [lo, hi]
+    return out
+
+
+def exact_axis_heading(k: int, direction: str, angle_min: float = ANGLE_MIN, angle_inc: float = ANGLE_INC):
+    """A heading h in [-pi, pi] with (h + angle_min) + k * angle_inc == AXIS_ANGLES[direction] in double, or None"""
+    target = AXIS_ANGLES[direction]
+    a = k * angle_inc
+    for b in _ulp_steps(target - a, 2):
+        if b + a != target:
+            continue
+        for h in _ulp_steps(b - angle_min, 3):
+            if h + angle_min == b and -math.pi <= h <= math.pi:
+                return h
+    return None
+
+
+def exact_axis_beams(direction: str, n_beams: int = N_BEAMS) -> list:
+    """[(beam index, heading)] of every beam that a heading puts exactly on the axis direction"""
+    out = []
+    for k in range(n_beams):
+        h = exact_axis_heading(k, direction)
+        if h is not None:
+            out.append((k, h))
+    return out
+
+
+def axis_scan(sensor_xy, direction: str, readings, n_beams: int = N_BEAMS, which: int = 0) -> tuple:
+    """(ranges, pose) of one scan whose exact-axis beams point along `direction` from sensor_xy.  readings = the ranges of
+    the beams: only one beam of a scan can lie exactly on an axis, so readings[0] goes there and any further readings go to
+    the beams right after it (a few hundredths of a degree off the axis).  `which` picks one of the exact beams."""
+    k, h = exact_axis_beams(direction, n_beams)[which]
+    r = np.full(n_beams, np.inf)
+    readings = np.atleast_1d(np.asarray(readings, dtype=np.float64))
+    assert k + len(readings) <= n_beams
+    r[k:k + len(readings)] = readings
+    return r, np.array([float(sensor_xy[0]), float(sensor_xy[1]), h])
+
+
+def clipped_end(s: float, p: float, r: float, rt: float) -> float:
+    """AddScan's end of an over-range beam along one axis, rounded like the reference (no fused multiply-add):
+    s + (rt / r) * (p - s)"""
+    return s + (rt / r) * (p - s)
+
+
+def clipped_end_fused(s: float, p: float, r: float, rt: float) -> float:
+    """the same end with s + ratio * dx fused into one rounding (exact rational arithmetic, rounded once)"""
+    from fractions import Fraction
+    ratio, dx = rt / r, p - s
+    return float(Fraction(s) + Fraction(ratio) * Fraction(dx))
+
+
+def grid_cell(w: float, offset: float, scale: float) -> int:
+    """CoordinateConverter::WorldToGrid on one axis: round half away from zero of (w - offset) * scale"""
+    v = (w - offset) * scale
+    return int(math.floor(v + 0.5) if v >= 0.0 else math.ceil(v - 0.5))
+
+
+def fma_sensitive_beams(boundary: float, offset: float, resolution: float, rt: float, n: int, seed: int, direction: str = "+x",
+                        max_r: float = RANGE_MAX) -> list:
+    """n (sensor coordinate, range) pairs of over-range axis beams (rt < r < max_r) whose clipped end lands in a different
+    grid cell when s + ratio * dx is fused: sensor coordinates step by units in the last place around boundary -+ rt."""
+    rng = np.random.default_rng(seed)
+    scale = 1.0 / resolution
+    sign = 1.0 if direction in ("+x", "+y") else -1.0
+    s0 = boundary - sign * rt
+    out, seen = [], set()
+    steps = _ulp_steps(s0, 64)
+    while len(out) < n:
+        s = steps[int(rng.integers(len(steps)))]
+        r = float(rng.uniform(rt * 1.0001, max_r * 0.999))
+        p = s + sign * r
+        e, f = clipped_end(s, p, r, rt), clipped_end_fused(s, p, r, rt)
+        if grid_cell(e, offset, scale) != grid_cell(f, offset, scale) and (s, r) not in seen:
+            seen.add((s, r))
+            out.append((s, r))
+    return out

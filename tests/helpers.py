@@ -105,3 +105,48 @@ def assert_occupancy_equals_golden(g, z, name):
     assert [int(g["passes"].sum()), int(g["hits"].sum())] == list(z[f"{name}/sums"])
     assert sha(g["passes"].astype(np.uint32)) == z[f"{name}/pass_sha"][0]
     assert sha(g["hits"].astype(np.uint32)) == z[f"{name}/hits_sha"][0]
+
+
+# b200_scan (include/b200slam.h) and kp_scan (oracle/karto_port.h) share this layout: int32 n, two pointers, double[3] pose
+SCAN_DTYPE = np.dtype([("n", "<i4"), ("pad", "<i4"), ("ranges", "<u8"), ("points_xy", "<u8"), ("sensor_pose", "<f8", (3,))])
+
+
+def scan_records(ranges, points, counts, poses):
+    """One scan record per scan over flat buffers (ragged stores): scan s is the counts[s] readings that start at
+    sum(counts[:s]) of ranges (B,) and points (B, 2).  The caller keeps the buffers alive."""
+    counts = np.asarray(counts, dtype=np.int64)
+    start = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.uint64)
+    assert ranges.flags.c_contiguous and points.flags.c_contiguous and ranges.dtype == points.dtype == np.float64
+    assert len(ranges) == counts.sum() and points.shape == (len(ranges), 2)
+    rec = np.zeros(max(len(counts), 1), dtype=SCAN_DTYPE)[:len(counts)]
+    rec["n"] = counts
+    rec["ranges"] = np.uint64(ranges.ctypes.data) + np.uint64(8) * start
+    rec["points_xy"] = np.uint64(points.ctypes.data) + np.uint64(16) * start
+    rec["sensor_pose"] = np.asarray(poses, dtype=np.float64).reshape(len(counts), 3)
+    return rec
+
+
+def port_occupancy(rec, res, rt, mp=2, th=0.1):
+    """kp_occupancy_create (the C port) on scan_records: dict(width, height, stride, offset, cells, passes, hits)"""
+    import ctypes as C
+    from oracle import karto_port as P
+    assert C.sizeof(P.KpScan) == SCAN_DTYPE.itemsize
+    h = P.lib().kp_occupancy_create(rec.ctypes.data_as(C.POINTER(P.KpScan)), len(rec), res, rt, LASER["min_range"],
+                                    LASER["max_range"], int(mp), th)
+    info = (C.c_int32 * 3)()
+    off = np.zeros(2)
+    P.lib().kp_occupancy_info(h, info, off.ctypes.data_as(C.POINTER(C.c_double)))
+    w, hh, st = info[0], info[1], info[2]
+    n = hh * st
+    grab = lambda f, t: np.ctypeslib.as_array(f(h), shape=(max(n, 1),))[:n].reshape(hh, st).astype(t, copy=True)   # noqa: E731
+    out = dict(width=w, height=hh, stride=st, offset=off, cells=grab(P.lib().kp_occupancy_cells, np.uint8),
+               passes=grab(P.lib().kp_occupancy_pass, np.uint32), hits=grab(P.lib().kp_occupancy_hits, np.uint32))
+    P.lib().kp_occupancy_destroy(h)
+    return out
+
+
+def occupancy_params(params):
+    """(resolution, range threshold, min_pass_through, occupancy_threshold) of a fixture's params row; negative = the
+    reference's defaults (2, 0.1)"""
+    res, rt, mp, th = (float(v) for v in params)
+    return res, rt, 2 if mp < 0 else int(mp), 0.1 if th < 0 else th
