@@ -175,6 +175,9 @@ int b200sm_batch_info(b200sm * h, int32_t info[8]);
 /* Plan of the tiled cluster kernel for the uploaded sweep: info = {available, cluster size (CTAs per pair), angle chunks,
  * sub-grid bands per parity phase, rows per band, refusal reason, resident clusters, shared memory per CTA (KB)}. */
 int b200sm_batch_tile_info(b200sm * h, int32_t info[8]);
+/* Pose-window tiling of the tiled cluster kernel (zero when it was refused): layout = {rows per y-tile (48: six row tiles of 8;
+ * 40: five, the window's last row then runs as a tail row), y-tiles, x-tiles, tail row (1 / 0)}. */
+int b200sm_batch_tile_layout(b200sm * h, int32_t layout[4]);
 /* What the tiled kernel's descriptor blocks hold for the uploaded sweep (host-side counts, zero when the tiled kernel was
  * refused): stats = {descriptor blocks, continuation sub-blocks (a stage's angles split over several staging buffers), largest
  * EDGE group (beams), (angle, phase, band, alignment) groups cut into more than one item, multi entries (cell, multiplicity),

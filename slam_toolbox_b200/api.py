@@ -115,6 +115,7 @@ def lib():
     L.b200sm_batch_winners_select.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int64), _DP, _DP, _DP]
     L.b200sm_batch_tile_info.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_tile_stats.argtypes = [C.c_void_p, _IP]
+    L.b200sm_batch_tile_layout.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_fetch_stats.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_upload_timing.argtypes = [C.c_void_p, _DP]
     L.b200sm_batch_reduce_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
@@ -391,8 +392,11 @@ class ScanMatcher:
         """Plan of the tiled cluster kernel for the uploaded sweep (b200sm_batch_tile_info)."""
         info = np.zeros(8, dtype=np.int32)
         _check(lib().b200sm_batch_tile_info(self._h, _ip(info)))
+        lay = np.zeros(4, dtype=np.int32)
+        _check(lib().b200sm_batch_tile_layout(self._h, _ip(lay)))
         return dict(available=bool(info[0]), cluster=int(info[1]), chunks=int(info[2]), bands=int(info[3]), band_rows=int(info[4]),
-                    refused_reason=int(info[5]), clusters=int(info[6]), smem_kb=int(info[7]))
+                    refused_reason=int(info[5]), clusters=int(info[6]), smem_kb=int(info[7]), ytile_rows=int(lay[0]),
+                    ytiles=int(lay[1]), xtiles=int(lay[2]), tail=bool(lay[3]))
 
     def batch_tile_stats(self):
         """What the tiled kernel's descriptor blocks hold for the uploaded sweep (b200sm_batch_tile_stats)."""

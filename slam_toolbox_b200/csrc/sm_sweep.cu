@@ -976,6 +976,7 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   // limit: 387 k vs 273 k matches/s at cfg2, bench.py); "sweep_kernel" = 1 still selects the single-CTA kernel.
   S.fast.enabled = 0; S.tile.enabled = 0;
   S.fast_info[0] = 0; S.tile_info[0] = 0;
+  for (int i = 0; i < 4; ++i) S.tile_layout[i] = 0;
   const auto t_tab0 = std::chrono::steady_clock::now();
   bool have = false;
   if (!h->force_generic && h->sweep_kernel == 1) have = build_fast_tables(h, S, st);
@@ -1551,6 +1552,13 @@ int b200sm_batch_tile_info(b200sm * h, int32_t info[8])
 {
   if (!h || !info || !h->sweep.uploaded) return B200_ERR_INVALID_ARG;
   for (int i = 0; i < 8; ++i) info[i] = h->sweep.tile_info[i];
+  return B200_OK;
+}
+
+int b200sm_batch_tile_layout(b200sm * h, int32_t layout[4])
+{
+  if (!h || !layout || !h->sweep.uploaded) return B200_ERR_INVALID_ARG;
+  for (int i = 0; i < 4; ++i) layout[i] = h->sweep.tile_layout[i];
   return B200_OK;
 }
 

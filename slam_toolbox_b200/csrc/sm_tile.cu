@@ -40,9 +40,11 @@
 
 namespace b200 {
 
-constexpr int kRowTiles = 6;           // row tiles of 8 rows per thread: one y-tile = 48 poses
-constexpr int kYTile = 8 * kRowTiles;
+constexpr int kRowTiles = 6;           // register pairs of 16-bit fields per thread: six row tiles of 8 rows (48-row y-tiles), or
+                                       // five (40-row y-tiles) + the tail row nY - 1 (see k_sweep_tile)
 constexpr int kChunkBeams = 640;       // beams accumulated in 16-bit fields before a flush (640 * 100 < 65536)
+constexpr int kMaxSingles = 63;        // weighted singles of one item (6-bit field of the item record, sm_types.cuh)
+constexpr int kMaxPairs = 255;         // weighted pairs of one item (8-bit field)
 
 // ------------------------------------------------------------------------------------------
 // PTX helpers: mbarrier, bulk async copy (TMA 1-D), cluster barrier, distributed shared memory
@@ -202,9 +204,15 @@ __device__ unsigned long long g_tile_timers[kTmCount];
 // kPitchW = the sub-grid row pitch in words as a compile-time constant (0 = take it from TileDev): with a constant pitch the 24
 // loads of a 4-beam step address as [descriptor register + immediate]; with a run-time pitch every load costs an extra IMAD
 // (20 % of the beam loop).  The pitches of the four shipped geometry combinations are instantiated.
-template <int kPitchW>
+// kTail = the y-tile layout (TileDev.tail): false = 48-row y-tiles of six row tiles; true = 40-row y-tiles of five row tiles, and in
+// the last y-tile the sixth register pair holds the tail row nY - 1, read lane-parallel over the entries (lane-row y_l takes every
+// 8th entry from the y_l-th on) and summed over the lane-rows at the flush.  A 2k + 1-row window (41, 81) then loads 40 k rows + an
+// eighth of a row per entry instead of 48 * ceil((2k + 1) / 48) rows.
+template <int kPitchW, bool kTail>
 __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, TileDev f)
 {
+  constexpr int kMain = kTail ? kRowTiles - 1 : kRowTiles;   // row tiles of 8 rows per y-tile
+  constexpr int kYTile = 8 * kMain;
   extern __shared__ __align__(128) unsigned char s_raw[];
   __shared__ TileShared sh;
   uint32_t * S = reinterpret_cast<uint32_t *>(s_raw);
@@ -345,13 +353,18 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         item = __shfl_sync(0xffffffffu, item, 0);
         if (item >= e.nitems) break;
         const uint2 rec = items[item];
-        int b = (int)(rec.x & 0xFFFFu);
-        const int pe = (int)(rec.x >> 16), me = pe + 2 * (int)(rec.y & 0xFFu);   // plain [b, pe), multi pairs [pe, me)
+        const int b0 = (int)(rec.x & 0xFFFFu);
+        int b = b0;
+        // plain beams [b0, pe), weighted singles [pe, se) (offset, weight), weighted pairs [ps, pe2) (offset, offset, weight, 0)
+        const int pe = b0 + (int)((rec.x >> 16) & 0x3FFu), se = pe + 2 * (int)(rec.x >> 26);
+        const int ps = (se + 3) & ~3, pe2 = ps + 4 * (int)(rec.y & 0xFFu);
         const int al = (int)((rec.y >> 8) & 63u), m = (int)((rec.y >> 14) & 3u);
         const int xt = (int)((rec.y >> 16) & 63u), yt = (int)((rec.y >> 22) & 255u);
         const int a = e.a0 + al;
         int32_t * Arow = A + (size_t)(a - chunk_a0) * P;
         const int ybase = y_l + kYTile * yt;
+        const int y_end = kTail ? nY - 1 : nY;          // rows of the main row tiles
+        const bool tail = kTail && yt == f.ytiles - 1;  // this y-tile also holds the tail row (warp-uniform)
        {
         int eb = 0, ee = 0;
         if (rec.y >> 31) {
@@ -360,10 +373,18 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         }
         uint32_t base = smem_u32(S8) + (uint32_t)(((y_l + kYTile * yt) * pitch_w + 4 * xt + j_l) * 4);   // shared-window address
         asm volatile("" : "+r"(base));   // one opaque register: every descriptor then costs PRMT + IMAD (no re-association of the sum)
-        // Idle lanes of the last y-tile (rows beyond the last pose) read past the band's nY-row halo, at most 47 rows into the
-        // accumulator region that follows S in shared memory: in bounds, and their sums are dropped at the flush (y >= nY) --
-        // so a band needs a halo of nY rows, not of whole y-tiles, and the row offsets stay warp-uniform (LDS [R + UR]).
+        // Idle lanes of the last y-tile (rows beyond the last pose) read past the band's nY-row halo, at most 47 rows (48-row
+        // y-tiles; 39 on the tail layout) into the accumulator region that follows S in shared memory: in bounds, and their sums
+        // are dropped at the flush (y >= y_end) -- so a band needs a halo of nY rows, not of whole y-tiles, and the row offsets
+        // stay warp-uniform (LDS [R + UR]).
         const int x0 = 4 * (4 * xt + j_l) - m;
+        auto add4 = [&](int32_t * dst, uint32_t t0, uint32_t t1) {
+          const int v0 = t0 & 0xFFFF, v1 = t1 & 0xFFFF, v2 = t0 >> 16, v3 = t1 >> 16;
+          if (v0 && (unsigned)(x0 + 0) < (unsigned)nX) atomicAdd(dst + 0, v0);
+          if (v1 && (unsigned)(x0 + 1) < (unsigned)nX) atomicAdd(dst + 1, v1);
+          if (v2 && (unsigned)(x0 + 2) < (unsigned)nX) atomicAdd(dst + 2, v2);
+          if (v3 && (unsigned)(x0 + 3) < (unsigned)nX) atomicAdd(dst + 3, v3);
+        };
         auto flush = [&](const uint32_t (&T0)[kRowTiles], const uint32_t (&T1)[kRowTiles]) {
           TILE_TM(kTmCorr);
           uint32_t any = 0;
@@ -371,20 +392,26 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
           for (int r = 0; r < kRowTiles; ++r) any |= T0[r] | T1[r];
           if (!__any_sync(0xffffffffu, any != 0)) { TILE_TM(kTmFlush); return; }
 #pragma unroll
-          for (int r = 0; r < kRowTiles; ++r) {
+          for (int r = 0; r < kMain; ++r) {
             const int y = ybase + 8 * r;
-            if (y >= nY || (T0[r] | T1[r]) == 0) continue;
-            int32_t * dst = Arow + y * nX + x0;
-            const int v0 = T0[r] & 0xFFFF, v1 = T1[r] & 0xFFFF, v2 = T0[r] >> 16, v3 = T1[r] >> 16;
-            if (v0 && (unsigned)(x0 + 0) < (unsigned)nX) atomicAdd(dst + 0, v0);
-            if (v1 && (unsigned)(x0 + 1) < (unsigned)nX) atomicAdd(dst + 1, v1);
-            if (v2 && (unsigned)(x0 + 2) < (unsigned)nX) atomicAdd(dst + 2, v2);
-            if (v3 && (unsigned)(x0 + 3) < (unsigned)nX) atomicAdd(dst + 3, v3);
+            if (y >= y_end || (T0[r] | T1[r]) == 0) continue;
+            add4(Arow + y * nX + x0, T0[r], T1[r]);
+          }
+          if (tail) {
+            // the tail row's fields of the 8 lane-rows of a word column: three butterfly adds (the item's whole weight fits
+            // 16 bits), lane-row 0 adds them
+            uint32_t t0 = T0[kRowTiles - 1], t1 = T1[kRowTiles - 1];
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+              t0 += __shfl_xor_sync(0xffffffffu, t0, o);
+              t1 += __shfl_xor_sync(0xffffffffu, t1, o);
+            }
+            if (y_l == 0 && (t0 | t1) != 0) add4(Arow + (nY - 1) * nX + x0, t0, t1);
           }
           TILE_TM(kTmFlush);
         };
-        // an item's plain and multi beams weigh at most kChunkBeams (the host splits longer groups): one flush
-        if (b < me) {
+        // an item's plain and weighted beams weigh at most kChunkBeams (the host splits longer groups): one flush
+        if (b < se || ps < pe2) {
           uint32_t T0[kRowTiles], T1[kRowTiles];
 #pragma unroll
           for (int r = 0; r < kRowTiles; ++r) { T0[r] = 0; T1[r] = 0; }
@@ -394,7 +421,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
             const uint32_t o0 = base + 4u * __byte_perm(dd.x, 0, 0x4410), o1 = base + 4u * __byte_perm(dd.x, 0, 0x4432);
             const uint32_t o2 = base + 4u * __byte_perm(dd.y, 0, 0x4410), o3 = base + 4u * __byte_perm(dd.y, 0, 0x4432);
 #pragma unroll
-            for (int r = 0; r < kRowTiles; ++r) {
+            for (int r = 0; r < kMain; ++r) {
               const uint32_t wa = lds_u32(o0 + r * 8 * pitchB) +
                                   lds_u32(o1 + r * 8 * pitchB);
               const uint32_t wb = lds_u32(o2 + r * 8 * pitchB) +
@@ -407,7 +434,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
             const uint32_t dd = *reinterpret_cast<const uint32_t *>(pay + b);
             const uint32_t o0 = base + ((dd & 0xFFFFu) << 2), o1 = base + ((dd >> 16) << 2);
 #pragma unroll
-            for (int r = 0; r < kRowTiles; ++r) {
+            for (int r = 0; r < kMain; ++r) {
               const uint32_t w = lds_u32(o0 + r * 8 * pitchB) +
                                  lds_u32(o1 + r * 8 * pitchB);
               T0[r] += even_bytes_t(w);
@@ -417,25 +444,63 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
           if (b < pe) {
             const uint32_t o0 = base + ((uint32_t)pay[b] << 2);
 #pragma unroll
-            for (int r = 0; r < kRowTiles; ++r) {
+            for (int r = 0; r < kMain; ++r) {
               const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
               T0[r] += even_bytes_t(w);
               T1[r] += odd_bytes_t(w);
             }
             ++b;
           }
-          // beams that share one grid cell: one load, fields times k (the host only builds multi entries when the whole
-          // group's weight fits one flush)
-          for (int k = pe; k < me; k += 2) {
+          // cells that k beams of the group share: one entry of weight k.  Two entries of equal weight are one pair: two loads
+          // added byte-wise (cell values <= 100), then one multiply-add per field; a weight without a partner is a single.
+          // (The host only builds weighted entries when the whole group's weight fits one flush.)
+          for (int k = pe; k < se; k += 2) {
             const uint32_t dm = *reinterpret_cast<const uint32_t *>(pay + k);
             const uint32_t o0 = base + ((dm & 0xFFFFu) << 2);
             const uint32_t kk = dm >> 16;
 #pragma unroll
-            for (int r = 0; r < kRowTiles; ++r) {
+            for (int r = 0; r < kMain; ++r) {
               const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
               T0[r] += even_bytes_t(w) * kk;
               T1[r] += odd_bytes_t(w) * kk;
             }
+          }
+          for (int k = ps; k < pe2; k += 4) {
+            const uint2 dp = *reinterpret_cast<const uint2 *>(pay + k);
+            const uint32_t o0 = base + 4u * __byte_perm(dp.x, 0, 0x4410), o1 = base + 4u * __byte_perm(dp.x, 0, 0x4432);
+            const uint32_t kk = dp.y;
+#pragma unroll
+            for (int r = 0; r < kMain; ++r) {
+              const uint32_t w = lds_u32(o0 + r * 8 * pitchB) +
+                                 lds_u32(o1 + r * 8 * pitchB);
+              T0[r] += even_bytes_t(w) * kk;
+              T1[r] += odd_bytes_t(w) * kk;
+            }
+          }
+          if (tail) {
+            // the tail row nY - 1, lane-parallel over the entries: lane-row y_l reads entry y_l, y_l + 8, ... (its descriptor
+            // with one LDS.U16 / LDS.32 / LDS.64 from 8 neighbouring entries, then the tail word of its column)
+            const uint32_t tb = smem_u32(S8) + (uint32_t)(((nY - 1) * pitch_w + 4 * xt + j_l) * 4);
+            uint32_t t0 = 0, t1 = 0;
+            for (int k = b0 + y_l; k < pe; k += 8) {
+              const uint32_t w = lds_u32(tb + ((uint32_t)pay[k] << 2));
+              t0 += even_bytes_t(w);
+              t1 += odd_bytes_t(w);
+            }
+            for (int k = pe + 2 * y_l; k < se; k += 16) {
+              const uint32_t dm = *reinterpret_cast<const uint32_t *>(pay + k);
+              const uint32_t w = lds_u32(tb + ((dm & 0xFFFFu) << 2));
+              t0 += even_bytes_t(w) * (dm >> 16);
+              t1 += odd_bytes_t(w) * (dm >> 16);
+            }
+            for (int k = ps + 4 * y_l; k < pe2; k += 32) {
+              const uint2 dp = *reinterpret_cast<const uint2 *>(pay + k);
+              const uint32_t w = lds_u32(tb + 4u * __byte_perm(dp.x, 0, 0x4410)) + lds_u32(tb + 4u * __byte_perm(dp.x, 0, 0x4432));
+              t0 += even_bytes_t(w) * dp.y;
+              t1 += odd_bytes_t(w) * dp.y;
+            }
+            T0[kRowTiles - 1] = t0;
+            T1[kRowTiles - 1] = t1;
           }
           flush(T0, T1);
         }
@@ -452,14 +517,21 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
             const int32_t mine = (lane < cn) ? f.edge[b0 + lane] : 0;
             for (int k = 0; k < cn; ++k) {
               const int32_t ev = __shfl_sync(0xffffffffu, mine, k);
-              const int row0 = (int)(int16_t)(ev & 0xFFFF) + ybase, wq = (ev >> 16) + 4 * xt + j_l;
+              const int rowb = (int)(int16_t)(ev & 0xFFFF), wq = (ev >> 16) + 4 * xt + j_l;
+              const int row0 = rowb + ybase;
               const bool cv = (unsigned)wq < (unsigned)pitch_w;
 #pragma unroll
-              for (int r = 0; r < kRowTiles; ++r) {
+              for (int r = 0; r < kMain; ++r) {
                 const int row = row0 + 8 * r;
                 const uint32_t w = (cv && (unsigned)row < (unsigned)f.alloc_rows) ? S[row * pitch_w + wq] : 0u;
                 T0[r] += even_bytes_t(w);
                 T1[r] += odd_bytes_t(w);
+              }
+              if (tail) {   // the tail row in lane-row 0 only (the flush sums the lane-rows)
+                const int row = rowb + nY - 1;
+                const uint32_t w = (y_l == 0 && cv && (unsigned)row < (unsigned)f.alloc_rows) ? S[row * pitch_w + wq] : 0u;
+                T0[kRowTiles - 1] += even_bytes_t(w);
+                T1[kRowTiles - 1] += odd_bytes_t(w);
               }
             }
           }
@@ -731,16 +803,21 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
 // host side: plan (chunks, bands, cluster size), descriptor blocks, launch
 // ------------------------------------------------------------------------------------------
 // the instantiation for a row pitch: 4 m / 12 m -> 76 words, 8 m / 12 m -> 92, 4 m / 20 m -> 116, 8 m / 20 m -> 132; anything else
-// runs the run-time-pitch version
-static const void * tile_kernel_for(int pitch_w)
+// runs the run-time-pitch version; each in both y-tile layouts
+template <bool kTail>
+static const void * tile_kernel_for_layout(int pitch_w)
 {
   switch (pitch_w) {
-    case 76: return (const void *)k_sweep_tile<76>;
-    case 92: return (const void *)k_sweep_tile<92>;
-    case 116: return (const void *)k_sweep_tile<116>;
-    case 132: return (const void *)k_sweep_tile<132>;
-    default: return (const void *)k_sweep_tile<0>;
+    case 76: return (const void *)k_sweep_tile<76, kTail>;
+    case 92: return (const void *)k_sweep_tile<92, kTail>;
+    case 116: return (const void *)k_sweep_tile<116, kTail>;
+    case 132: return (const void *)k_sweep_tile<132, kTail>;
+    default: return (const void *)k_sweep_tile<0, kTail>;
   }
+}
+static const void * tile_kernel_for(int pitch_w, bool tail)
+{
+  return tail ? tile_kernel_for_layout<true>(pitch_w) : tile_kernel_for_layout<false>(pitch_w);
 }
 
 static int env_int(const char * name, int dflt)
@@ -754,24 +831,43 @@ static inline bool d_max_n_ok(int max_n) { return max_n > 0 && (max_n & 3) == 0 
 
 static inline int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
+// Reorders a sorted descriptor list so that entries i, i + 1, ..., i + 7 (what the 8 lane-rows read at once for the tail row) come
+// from 8 spread-out parts of the sorted order: neighbouring cells would put their 4-word runs on the same banks.  The sums are
+// integers, so the order is free.
+static void spread_rows(std::vector<uint16_t>::iterator b, std::vector<uint16_t>::iterator e)
+{
+  const size_t L = (size_t)(e - b), R = (L + 7) / 8;
+  if (L < 9) return;
+  const std::vector<uint16_t> src(b, e);
+  size_t o = 0;
+  for (size_t j = 0; j < R; ++j)
+    for (size_t y = 0; y < 8; ++y)
+      if (y * R + j < L) b[o++] = src[y * R + j];
+}
+
 // The warp items of one descriptor block, longest first (the shared queue then hands out long items first).  tbl holds (plain
-// begin, multi begin, multi end) per (angle, alignment) group, nedge the group's EDGE beams.  A group's plain list is cut into
-// pieces of at most kChunkBeams beams (4-aligned starts: the 4-beam step reads descriptors with 64-bit loads), so that every item
-// flushes its 16-bit fields once; the multi pairs and the EDGE beams go with the last piece.
-static void build_block_items(const std::vector<int32_t> & tbl, const std::vector<int> & nedge, int na, int xtiles, int ytiles,
+// begin, singles begin, singles end, pairs end) per (angle, alignment) group (the pairs begin at the first 4-entry boundary from the
+// singles' end), nedge the group's EDGE beams.  A group's plain list is cut into pieces of at most kChunkBeams beams (4-aligned
+// starts: the 4-beam step reads descriptors with 64-bit loads), so that every item flushes its 16-bit fields once; the weighted
+// singles and pairs and the EDGE beams go with the last piece.
+// Returns false when a piece does not fit its record's fields (the encoder keeps them in range: a planner refusal, not a wrap).
+static bool build_block_items(const std::vector<int32_t> & tbl, const std::vector<int> & nedge, int na, int xtiles, int ytiles,
                               std::vector<uint2> & out)
 {
-  struct Piece { int work; int pb, pe, mpairs, al, m; bool edge; };
+  struct Piece { int work; int pb, pe, nsingle, npair, al, m; bool edge; };
   std::vector<Piece> pieces;
   for (int g = 0; g < na * 4; ++g) {
-    const int pb = tbl[3 * g], mb = tbl[3 * g + 1], mpairs = (tbl[3 * g + 2] - mb) / 2, ne = nedge[g];
-    if (mb == pb && mpairs == 0 && ne == 0) continue;
+    const int pb = tbl[4 * g], sb = tbl[4 * g + 1], se = tbl[4 * g + 2], pe2 = tbl[4 * g + 3];
+    const int ns = (se - sb) / 2, np = pe2 > se ? (pe2 - ((se + 3) & ~3)) / 4 : 0;
+    const int ne = nedge[g];
+    if (sb == pb && ns == 0 && np == 0 && ne == 0) continue;
     for (int s = pb;; s += kChunkBeams) {
-      Piece p{0, s, std::min(mb, s + kChunkBeams), 0, g >> 2, g & 3, false};
-      if (p.pe == mb) { p.mpairs = mpairs; p.edge = ne > 0; }
-      p.work = (p.pe - p.pb) + p.mpairs + (p.edge ? ne : 0);
+      Piece p{0, s, std::min(sb, s + kChunkBeams), 0, 0, g >> 2, g & 3, false};
+      if (p.pe == sb) { p.nsingle = ns; p.npair = np; p.edge = ne > 0; }
+      p.work = (p.pe - p.pb) + p.nsingle + 2 * p.npair + (p.edge ? ne : 0);   // entries loaded
+      if (p.pb > 0xFFFF || p.pe - p.pb > 0x3FF || p.nsingle > kMaxSingles || p.npair > kMaxPairs) return false;
       pieces.push_back(p);
-      if (p.pe == mb) break;
+      if (p.pe == sb) break;
     }
   }
   std::stable_sort(pieces.begin(), pieces.end(), [](const Piece & x, const Piece & y) { return x.work > y.work; });
@@ -779,9 +875,10 @@ static void build_block_items(const std::vector<int32_t> & tbl, const std::vecto
   for (const Piece & p : pieces)
     for (int yt = 0; yt < ytiles; ++yt)
       for (int xt = 0; xt < xtiles; ++xt)
-        out.push_back(make_uint2((uint32_t)p.pb | ((uint32_t)p.pe << 16),
-                                 (uint32_t)p.mpairs | ((uint32_t)p.al << 8) | ((uint32_t)p.m << 14) | ((uint32_t)xt << 16) |
+        out.push_back(make_uint2((uint32_t)p.pb | ((uint32_t)(p.pe - p.pb) << 16) | ((uint32_t)p.nsingle << 26),
+                                 (uint32_t)p.npair | ((uint32_t)p.al << 8) | ((uint32_t)p.m << 14) | ((uint32_t)xt << 16) |
                                    ((uint32_t)yt << 22) | (p.edge ? 0x80000000u : 0u)));
+  return true;
 }
 
 bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
@@ -792,6 +889,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   TileDev & T = S.tile;
   T = TileDev{};
   for (int i = 0; i < 8; ++i) S.tile_info[i] = 0;
+  for (int i = 0; i < 4; ++i) S.tile_layout[i] = 0;
   for (int i = 0; i < 8; ++i) S.tile_stats[i] = 0;
   auto bail = [&](int why) {
     for (int i = 0; i < 8; ++i) S.tile_stats[i] = 0;
@@ -801,8 +899,13 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   // Packed fields and their bounds (a refusal runs the sweep on the generic kernel, which takes any n and nA):
   //   TileSeq.a0 / chunk (int16)   nA <= 4096                                                  -> 2
   //   item al (6 bits)             nAc <= 63 angles per chunk (the V loop)                     -> 4 when no V fits
-  //   item mpairs (8 bits)         multi entries only in groups of <= kChunkBeams beams: <= 214   (no refusal needed)
-  //   one angle's block            payload <= n + 16 entries, records per the one_angle minimum  -> 8
+  //   item plain count (10 bits)   pieces of <= kChunkBeams = 640 beams
+  //   item singles (6 bits)        weighted entries only in groups of <= kChunkBeams beams: one single per distinct weight
+  //                                k >= 2 (2 + 3 + ... + 36 = 665 > 640: <= 34 weights) + the odd plain beam: <= 35; without
+  //                                pairing (B200_TILE_PAIRS=0) the encoder returns singles beyond 62 to the plain list
+  //   item pairs (8 bits)          a pair weighs >= 4 beams: <= 640 / 4 = 160 per group
+  //   (all three, and pb, are checked per record by build_block_items)                        -> 13
+  //   one angle's block            payload <= n + 32 entries, records per the one_angle minimum  -> 8
   //   TileSeq.nitems (int16)       records of one block                                        -> 10
   //   item pb / pe (16 bits)       payload entries of one block                                -> 11
   //   TileSeq.off (int32)          descriptor blob bytes                                       -> 12
@@ -817,7 +920,15 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   // ---- geometry of one parity sub-grid ----
   int pitch_w = (g.stride / 2 + 16 + 3) / 4;             // sub-grid row + the 3-word overhang of the last x-tile
   while ((pitch_w & 7) != 4) ++pitch_w;                  // 8 rows x 4 words of a warp hit 32 distinct banks
-  const int xtiles = (nX + 3 + 15) / 16, ytiles = (nY + kYTile - 1) / kYTile;
+  // y-tile layout, by the row-tile loads of one beam and x-tile (in eighths of a row tile): 48-row y-tiles of six row tiles, or
+  // 40-row y-tiles of five + the tail row (one descriptor and one word load per 8 entries, i.e. 2 / 8).  41 rows: 42 vs 48; 81
+  // rows: 82 vs 96; 45 rows: 82 vs 48 (stays on 48-row tiles)
+  const int yt48 = (nY + 47) / 48, yt40 = std::max(1, (nY - 1 + 39) / 40);
+  // B200_TILE_TAIL=0 / B200_TILE_PAIRS=0 switch the tail layout / the weight-2 entries and pairing off, to measure each part alone
+  const bool tail = env_int("B200_TILE_TAIL", 1) != 0 && 8 * 5 * yt40 + 2 < 8 * 6 * yt48;
+  const bool pairs_on = env_int("B200_TILE_PAIRS", 1) != 0;
+  const int ytile_rows = tail ? 40 : 48;
+  const int xtiles = (nX + 3 + 15) / 16, ytiles = tail ? yt40 : yt48;
   if (xtiles > kItemMaxXTiles || ytiles > kItemMaxYTiles) return bail(9);
   const int rows_valid = (g.height + 1) / 2;
   const int halo = nY + 2;                               // rows a beam window reaches below its base row (idle row tiles are clamped) + the wrapped row
@@ -850,7 +961,9 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     // staging buffer: item list + 1.5 x the average descriptor bytes of a (chunk, phase) block, at least one angle's worst case:
     // one item record per (alignment, tile), plus one per tile for every further kChunkBeams-piece of a long group -- the
     // groups of one angle hold at most n beams, so they are cut at most (n - 1) / kChunkBeams more times
-    const int one_angle = 8 * xtiles * ytiles * (4 + std::max(n - 1, 0) / kChunkBeams) + 2 * n + 64;
+    // payload of one angle: <= 2 bytes per beam (a plain beam 2, a single of weight >= 2 4, a pair of weight >= 2 each 8) + per group
+    // <= 6 bytes of 4-entry alignment before the plain list, 2 for the odd plain beam's single, 4 before the pairs; + 6 at the end
+    const int one_angle = 8 * xtiles * ytiles * (4 + std::max(n - 1, 0) / kChunkBeams) + 2 * n + 4 * 12 + 6 + 10;
     int stage = 16 + nAc * 52 + (nAc * n * 2 * 3) / 8 + 64 * nAc;
     stage = std::max(stage, one_angle + 64);
     stage = (stage + 127) & ~127;
@@ -866,7 +979,9 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     // cost of one pair on one CTA, in thread-instructions: rasters (4 phases per chunk and band) + the beam loop per angle
     // the accumulator flush of every (angle, stage, alignment, tile) item (~100 warp instructions each, 32 warps) and the fixed
     // cost of a stage (clear + raster + three barriers) are what make extra bands expensive
-    const long w_angle = (long)((double)P * n * 0.8 / kTileThreads) + 4L * nbv * (4L * xtiles * ytiles * 100 / 32);
+    // the beam loop: ~2.3 thread-instructions per lane and row-tile load (6 per beam and 48-row y-tile; 5 + 2 / 8 with the tail)
+    const double loads = tail ? 5.0 * ytiles + 0.25 : 6.0 * ytiles;
+    const long w_angle = (long)((double)n * xtiles * loads * 32 * 2.3 / kTileThreads) + 4L * nbv * (4L * xtiles * ytiles * 100 / 32);
     const long w_raster = 4 * (700 + 3L * std::min(B + halo, rows_valid + halo - nY) * pitch_w / kTileThreads);
     const long cost = (long)((V + Cc - 1) / Cc) * (nbv * w_raster + nAc * w_angle);
     if (bestCost < 0 || cost < bestCost) { bestCost = cost; bestV = V; bestNb = nbv; bestB = B; bestStage = stage; }
@@ -879,7 +994,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   const size_t s_bytes = ((size_t)alloc_rows * pitch_w * 4 + 15) & ~(size_t)15;
   const size_t a_bytes = ((size_t)nAc * P * 4 + 15) & ~(size_t)15;
   T.C = C; T.V = V; T.nAc = nAc; T.nbands = nbands; T.band_rows = B; T.alloc_rows = alloc_rows; T.pitch_w = pitch_w;
-  T.xtiles = xtiles; T.ytiles = ytiles; T.stage_bytes = stage_bytes;
+  T.xtiles = xtiles; T.ytiles = ytiles; T.tail = tail ? 1 : 0; T.stage_bytes = stage_bytes;
   T.int_ties = int_ties;
   {
     // distinct non-zero smear values, ascending; up to 4 -> levelled (atomic-free) raster
@@ -897,9 +1012,9 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   if (T.off_cells + 2 * (size_t)cell_cap * 4 + sizeof(TileShared) + 64 > 227 * 1024) cell_cap = 0;
   T.cell_cap = cell_cap;
   size_t smem = T.off_cells + 2 * (size_t)cell_cap * 4;
-  // idle lanes of the last y-tile read up to (48 ytiles - nY) rows past the band (see the kernel): keep those reads inside the
-  // allocation even when everything behind S is small (tiny search windows)
-  const size_t overrun = (size_t)(kYTile * ytiles - nY + 1) * pitch_w * 4;
+  // idle lanes of the last y-tile read up to (ytile_rows * ytiles - nY) rows past the band (see the kernel): keep those reads inside
+  // the allocation even when everything behind S is small (tiny search windows)
+  const size_t overrun = (size_t)std::max(ytile_rows * ytiles - nY + 1, 1) * pitch_w * 4;
   if (smem - s_bytes < overrun) smem = s_bytes + overrun;
   if (smem + sizeof(TileShared) + 64 > 227 * 1024) return bail(5);
 
@@ -915,7 +1030,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   std::vector<std::vector<uint16_t>> grp((size_t)nA * nstage * 4);
   std::vector<std::vector<int32_t>> egrp((size_t)nA * nstage * 4), wgrp((size_t)nA * nstage);
   blob.reserve((size_t)nq * nA * n * 2 + 4096);
-  struct Encoded { int32_t tbl[12]; std::vector<uint16_t> pay; };
+  struct Encoded { int32_t tbl[16]; std::vector<uint16_t> pay; };
   std::vector<Encoded> enc((size_t)nA * nstage);
   std::vector<std::vector<int32_t>> slow_a(nA);
   std::vector<int> nfast_a(nA), nedge_a(nA);
@@ -968,8 +1083,8 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
         }
       }
       nfast_a[a] = nf; nedge_a[a] = ne;
-      // the angle's groups of every stage: table of (plain begin, multi begin, multi end) per alignment, relative to the
-      // angle's own payload (whose start is 4-entry aligned in the block), and the payload
+      // the angle's groups of every stage: table of (plain begin, singles begin, pairs begin, pairs end) per alignment, relative
+      // to the angle's own payload (whose start is 4-entry aligned in the block), and the payload
       for (int sg = 0; sg < nstage; ++sg) {
         Encoded & E = enc[(size_t)a * nstage + sg];
         std::vector<uint16_t> & pay = E.pay;
@@ -979,28 +1094,55 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
           std::sort(gk.begin(), gk.end());
           while (pay.size() & 3) pay.push_back(0);   // the plain list is read with 64-bit loads
           const int pb = (int)pay.size();
-          // run-length encode: beams that land in the same cell share a descriptor.  Entries with multiplicity >= 3 go to the
-          // group's multi list (one load, fields multiplied), provided the whole group fits one flush.
+          // run-length encode: beams that land in the same cell share one entry of weight k (one load per row, fields times
+          // k), provided the whole group fits one flush.  Entries of equal weight are then paired (two loads added byte-wise,
+          // one multiply per field); weight-1 beams stay in the plain list.
           const bool dedup = !h->no_dedup && gk.size() <= (size_t)kChunkBeams;
-          std::vector<std::pair<uint16_t, uint16_t>> multi;
+          std::vector<std::pair<uint16_t, uint16_t>> multi;   // (weight, offset)
           for (size_t i = 0; i < gk.size();) {
             size_t j = i;
             while (j < gk.size() && gk[j] == gk[i]) ++j;
             const size_t cnt = j - i;
-            if (dedup && cnt >= 3) multi.emplace_back(gk[i], (uint16_t)cnt);
+            if (dedup && cnt >= (pairs_on ? 2u : 3u)) multi.emplace_back((uint16_t)cnt, gk[i]);
             else for (size_t t = 0; t < cnt; ++t) pay.push_back(gk[i]);
             i = j;
           }
-          // the multi list (offset, multiplicity pairs, read as 32-bit words) starts where the plain list ends: keep that
-          // index even by moving an odd plain list's last entry into the multi list with multiplicity 1
+          std::stable_sort(multi.begin(), multi.end(),
+                           [](const std::pair<uint16_t, uint16_t> & x, const std::pair<uint16_t, uint16_t> & y) { return x.first < y.first; });
+          std::vector<std::pair<uint16_t, uint16_t>> single;   // (offset, weight)
+          std::vector<uint16_t> pairs;                         // offset, offset, weight, 0
+          for (size_t i = 0; i < multi.size();) {
+            if (pairs_on && i + 1 < multi.size() && multi[i + 1].first == multi[i].first) {
+              pairs.insert(pairs.end(), {multi[i].second, multi[i + 1].second, multi[i].first, (uint16_t)0});
+              i += 2;
+            } else {
+              single.emplace_back(multi[i].second, multi[i].first);
+              i += 1;
+            }
+          }
+          // the item record counts the singles in 6 bits.  With pairing there are at most 35 (see the field bounds); without it
+          // (B200_TILE_PAIRS=0) every merged cell is a single: those beyond kMaxSingles - 1 (one slot stays free for the odd plain
+          // beam below) go back to the plain list as k plain beams each
+          while (single.size() > (size_t)kMaxSingles - 1) {
+            for (uint16_t t = 0; t < single.back().second; ++t) pay.push_back(single.back().first);
+            single.pop_back();
+          }
+          // the tail row reads entries 8 apart in each lane-row: spread the plain list's neighbouring (sorted, so nearby)
+          // word offsets over the lane-rows so that their 4-word runs rarely share banks (48-row y-tiles have no tail row)
+          if (tail) spread_rows(pay.begin() + pb, pay.end());
+          // the singles (offset, weight; read as 32-bit words) start where the plain list ends: keep that index even by
+          // moving an odd plain list's last entry into the singles with weight 1
           if (((int)pay.size() - pb) & 1) {
             const uint16_t last = pay.back();
             pay.pop_back();
-            multi.emplace_back(last, (uint16_t)1);
+            single.emplace_back(last, (uint16_t)1);
           }
-          const int mb = (int)pay.size();
-          for (auto & mk : multi) { pay.push_back(mk.first); pay.push_back(mk.second); }
-          E.tbl[3 * m + 0] = pb; E.tbl[3 * m + 1] = mb; E.tbl[3 * m + 2] = (int)pay.size();
+          const int sb = (int)pay.size();
+          for (auto & s1 : single) { pay.push_back(s1.first); pay.push_back(s1.second); }
+          const int se = (int)pay.size();
+          if (!pairs.empty()) while (pay.size() & 3) pay.push_back(0);   // the pairs are read as 64-bit words
+          pay.insert(pay.end(), pairs.begin(), pairs.end());
+          E.tbl[4 * m + 0] = pb; E.tbl[4 * m + 1] = sb; E.tbl[4 * m + 2] = se; E.tbl[4 * m + 3] = (int)pay.size();
         }
         while (pay.size() & 3) pay.push_back(0);
       }
@@ -1041,7 +1183,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
             while (a + na < ca0 + cna) {
               const Encoded & E = enc[(size_t)(a + na) * nstage + sg];
               int ep = 0;
-              for (int m = 0; m < 4; ++m) ep += std::max(1, (E.tbl[3 * m + 1] - E.tbl[3 * m] + kChunkBeams - 1) / kChunkBeams);
+              for (int m = 0; m < 4; ++m) ep += std::max(1, (E.tbl[4 * m + 1] - E.tbl[4 * m] + kChunkBeams - 1) / kChunkBeams);
               const size_t hdr = (((size_t)(npieces + ep) * xtiles * ytiles * 8) + 15) & ~(size_t)15;
               const size_t bytes = (hdr + (pay.size() + E.pay.size()) * 2 + 15) & ~(size_t)15;
               const bool wide = pay.size() + E.pay.size() > 65535;   // item records hold 16-bit payload indices (pb, pe)
@@ -1050,24 +1192,26 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
                 return bail(wide ? 11 : 8);   // one angle does not fit the 16-bit indices / the staging buffer
               }
               const int shift = (int)pay.size();
-              for (int k = 0; k < 12; ++k) tbl.push_back(E.tbl[k] + shift);
+              for (int k = 0; k < 16; ++k) tbl.push_back(E.tbl[k] + shift);
               pay.insert(pay.end(), E.pay.begin(), E.pay.end());
               npieces += ep;
               ++na;
             }
             nedge.assign((size_t)na * 4, 0);
             for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)egrp[((size_t)(a + (g2 >> 2)) * nstage + sg) * 4 + (g2 & 3)].size();
-            build_block_items(tbl, nedge, na, xtiles, ytiles, items);
+            if (!build_block_items(tbl, nedge, na, xtiles, ytiles, items)) return bail(13);
             if (items.size() > 32767) return bail(10);   // TileSeq.nitems is 16-bit
             int32_t * ts = S.tile_stats;
             ts[0] += 1;
             ts[1] += first_sub ? 0 : 1;
             for (int g2 = 0; g2 < na * 4; ++g2) {
-              const int pb = tbl[3 * g2], mb = tbl[3 * g2 + 1], me = tbl[3 * g2 + 2];
+              const int pb = tbl[4 * g2], mb = tbl[4 * g2 + 1], se = tbl[4 * g2 + 2], pe2 = tbl[4 * g2 + 3];
+              const int ps = pe2 > se ? ((se + 3) & ~3) : se;
               ts[2] = std::max(ts[2], nedge[g2]);
               ts[3] += mb - pb > kChunkBeams ? 1 : 0;
-              ts[4] += (me - mb) / 2;
-              for (int k = mb; k < me; k += 2) ts[5] = std::max(ts[5], (int32_t)pay[k + 1]);
+              ts[4] += (se - mb) / 2 + (pe2 - ps) / 2;   // weighted entries: singles + both entries of every pair
+              for (int k = mb; k < se; k += 2) ts[5] = std::max(ts[5], (int32_t)pay[k + 1]);
+              for (int k = ps; k < pe2; k += 4) ts[5] = std::max(ts[5], (int32_t)pay[k + 2]);
               ts[6] = std::max(ts[6], mb - pb);
             }
             const size_t hdr = ((items.size() * 8) + 15) & ~(size_t)15;
@@ -1122,7 +1266,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   S.tile_smem = smem;
 
   // ---- grid: as many co-resident clusters as the device holds, one pair per cluster at a time ----
-  const void * kfn = tile_kernel_for(pitch_w);
+  const void * kfn = tile_kernel_for(pitch_w, T.tail != 0);
   B200_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int max_clusters = sms / C;
   {
@@ -1142,6 +1286,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   S.tile_grid = clusters * C;
   S.tile_info[0] = 1; S.tile_info[1] = C; S.tile_info[2] = V; S.tile_info[3] = nbands; S.tile_info[4] = B; S.tile_info[5] = 0;
   S.tile_info[6] = clusters; S.tile_info[7] = (int32_t)(smem / 1024);
+  S.tile_layout[0] = ytile_rows; S.tile_layout[1] = ytiles; S.tile_layout[2] = xtiles; S.tile_layout[3] = tail ? 1 : 0;
   S.fast_info[1] = n_fast; S.fast_info[2] = n_edge; S.fast_info[3] = (int32_t)slow.size() - 1;
   return true;
 }
@@ -1158,7 +1303,7 @@ void launch_sweep_tile(b200sm * h, SweepHost & S, cudaStream_t st)
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = (unsigned)S.tile.C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
-  const void * kfn = tile_kernel_for(S.tile.pitch_w);
+  const void * kfn = tile_kernel_for(S.tile.pitch_w, S.tile.tail != 0);
   B200_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S.tile_smem));
   void * args[] = {(void *)&S.dev, (void *)&S.tile};
   B200_CUDA(cudaLaunchKernelExC(&cfg, kfn, args));

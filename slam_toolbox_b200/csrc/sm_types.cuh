@@ -155,11 +155,14 @@ struct TileSeq {                 // one descriptor block of a query's schedule (
   int16_t nitems;                // warp items of this block (8-byte records at the start of the block, see below)
   uint32_t flags;                // kSeq* bits
 };
-// One warp item of a descriptor block (8 bytes, longest first): beams [pb, pe) of the payload's plain list and the
-// mpairs (offset, multiplicity) pairs that follow them, for the angle a0 + al, alignment m and tile (xt, yt).  Items of a
-// long group hold consecutive pieces of its plain list; the EDGE beams of a (group, tile) go with exactly one item (edge).
-//   x = pb | pe << 16;  y = mpairs | al << 8 | m << 14 | xt << 16 | yt << 22 | edge << 31
-// (al < 64: the planner's nAc <= 63; mpairs < 256: multi entries exist only in groups of at most kChunkBeams beams)
+// One warp item of a descriptor block (8 bytes, longest first), for the angle a0 + al, alignment m and tile (xt, yt): the np
+// plain beams [pb, pb + np) of the payload (16-bit word offsets), then ns weighted singles (offset, weight: one 32-bit word each)
+// and, from the next 4-entry boundary, npairs weighted pairs (offset, offset, weight, 0: one 64-bit word each; both cells of a pair
+// have the same weight).  A weight is the number of the group's beams that land in that cell.  Items of a long group hold
+// consecutive pieces of its plain list; the EDGE beams of a (group, tile) go with exactly one item (edge).
+//   x = pb | np << 16 | ns << 26;  y = npairs | al << 8 | m << 14 | xt << 16 | yt << 22 | edge << 31
+// (al < 64: the planner's nAc <= 63; np <= 640, ns <= 63, npairs <= 160: derived with the planner's refusal codes in sm_tile.cu,
+// and every record is checked against its field widths)
 constexpr int kItemMaxXTiles = 64, kItemMaxYTiles = 256;
 constexpr uint32_t kSeqNewChunk = 1, kSeqNewStage = 2, kSeqEndChunk = 4, kSeqHasWrap = 16;
 struct TileDev {
@@ -167,6 +170,7 @@ struct TileDev {
   int C, V, nAc;                 // cluster size, angle chunks, angles per chunk
   int nbands, band_rows, alloc_rows, pitch_w;   // sub-grid banding (rows of one parity), allocated rows, row pitch in words
   int xtiles, ytiles;
+  int tail;                      // y-tiles of 40 rows + the tail row nY - 1 in the last one (else 48-row y-tiles)
   int stage_bytes;               // size of one descriptor staging buffer
   int nlevels;                   // distinct non-zero smear-kernel values if <= 4 (levelled raster without atomics), else 0
   uint32_t level[4];             // ... ascending
@@ -216,6 +220,7 @@ struct SweepHost {
   // what the tiled kernel's descriptor blocks contain (b200sm_batch_tile_stats): blocks, continuation sub-blocks, largest EDGE
   // group, groups cut into pieces, multi entries, largest multiplicity, largest plain group, wrap2 entries
   int32_t tile_stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  int32_t tile_layout[4] = {0, 0, 0, 0};   // rows per y-tile (40 or 48), y-tiles, x-tiles, tail row (b200sm_batch_tile_layout)
   DevBuf<uint8_t> d_tile_desc;
   DevBuf<TileSeq> d_tile_seq;
   DevBuf<int32_t> d_tile_seq_start, d_tile_edge, d_tile_edge_start, d_tile_wrap2, d_tile_wrap2_start, d_tile_slow, d_tile_slow_start;

@@ -612,6 +612,48 @@ def make_highres_sweep(n_beams: int, fov_deg: float, *, seed: int = 11, n_querie
     return AdversarialSweep(qr, qpose, cr, cposes, chain_start, (amin, inc), (amin, inc))
 
 
+WEIGHTED_BEAMS = 8192   # laser of make_weighted_sweep: 360 deg at 0.044 deg
+
+
+def make_weighted_sweep(weights, *, resolution: float = 0.05, r_min: float = 1.5, r_max: float = 4.0,
+                        seed: int = 111) -> AdversarialSweep:
+    """One query whose beams land in chosen cells: cell i is hit by weights[i] neighbouring beams of a 8192-beam, 360 deg laser.
+    At the query's own heading (the central search angle) every cell is 8 columns x 2 rows apart on the query-centred cell
+    lattice, so they all fall in ONE (parity phase, alignment) descriptor group, whose weight is sum(weights); the other angles
+    shuffle them over the groups.  The cells lie r_min..r_max from the query (at most 12 mm off a cell centre at 4 m for a
+    weight of 10), the other readings are inf.  Candidates: chain 0 a room scan, chain 1 the query's own scan, chain 2 both."""
+    ls = make_loop_sweep(seed, n_queries=1, n_chains=2, chain_len=1)
+    q = ls.query_poses[0].copy()
+    q[2] = 0.0
+    amin, inc = highres_laser(WEIGHTED_BEAMS, 360.0)
+    lim = int(r_max / resolution) + 8
+    u = np.arange(-lim, lim + 1, 8)
+    v = np.arange(-lim, lim + 1, 2)
+    gx, gy = np.meshgrid(u, v)
+    pts = np.column_stack([gx.ravel(), gy.ravel()]) * resolution
+    rad = np.hypot(pts[:, 0], pts[:, 1])
+    pts, rad = pts[(rad >= r_min) & (rad <= r_max)], rad[(rad >= r_min) & (rad <= r_max)]
+    beam = np.rint((np.arctan2(pts[:, 1], pts[:, 0]) - amin) / inc).astype(int) % WEIGHTED_BEAMS
+    order = np.argsort(beam, kind="stable")
+    qr = np.full(WEIGHTED_BEAMS, np.inf)
+    nxt, k = 0, 0
+    for i in order:   # cells in bearing order, each on its own run of beams with one beam between runs
+        if k == len(weights):
+            break
+        w = int(weights[k])
+        b0 = beam[i] - w // 2
+        if b0 < nxt or b0 + w > WEIGHTED_BEAMS:
+            continue
+        qr[b0:b0 + w] = rad[i]
+        nxt, k = b0 + w + 1, k + 1
+    if k < len(weights):
+        raise ValueError(f"only {k} of {len(weights)} cells fit r_min..r_max")
+    room = raycast(ls.world, ls.cand_poses, n_beams=WEIGHTED_BEAMS, angle_min=amin, angle_inc=inc)
+    cr = np.concatenate([room[:1], qr[None, :], room[1:2], qr[None, :]])
+    cp = np.concatenate([ls.cand_poses[:1], q[None, :], ls.cand_poses[1:2], q[None, :]])
+    return AdversarialSweep(qr[None, :], q[None, :], cr, cp, np.array([0, 1, 2, 4], dtype=np.int32), (amin, inc), (amin, inc))
+
+
 def make_long_query_sweep(n: int, seed: int = 7, n_chains: int = 3, inf_frac: float = 0.97) -> AdversarialSweep:
     """One query of n beams over the usual 270 deg field of view (a room scan at n / 1081 times the angular density, a fraction
     inf_frac of the readings replaced by inf) and n_chains room-scan candidates.  With the defaults, n = 10240 and the 4 m /
