@@ -238,9 +238,14 @@ typedef struct b200pg_opts {
    * Other values are refused with B200_ERR_INVALID_ARG. */
   int32_t trust_region_strategy;
   int32_t dogleg_type;
+  /* linear solver of every trust-region step: 0 = the PCG kernels above (the default), 1 = exact block-sparse Cholesky
+   * (SPARSE_NORMAL_CHOLESKY, ceres_solver.cpp:96-97): an FP64 supernodal factorisation of (H + shift D^2) over the free
+   * nodes on the device, after a host analysis that is kept while the free nodes and their adjacent pairs stay the same.
+   * pcg_tolerance and pcg_max_iterations do not apply to it. Other values are refused with B200_ERR_INVALID_ARG. */
+  int32_t linear_solver_type;
 } b200pg_opts;
-/* b200pg_opts and b200pg_summary grew (trust_region_strategy, dogleg_type; linear_solves): the ctypes mirror
- * (slam_toolbox_b200/api.py PgOpts / PgSummary) and every compiled caller must be rebuilt against this header. */
+/* b200pg_opts and b200pg_summary grew (trust_region_strategy, dogleg_type, linear_solver_type; linear_solves): the ctypes
+ * mirror (slam_toolbox_b200/api.py PgOpts / PgSummary) and every compiled caller must be rebuilt against this header. */
 
 typedef struct b200pg_summary {
   int32_t iterations;          /* LM iterations (successful + unsuccessful)            */
@@ -255,9 +260,11 @@ typedef struct b200pg_summary {
   float wall_ms;               /* host wall time of the whole call                     */
   int32_t uploaded_edges;      /* constraints copied to the device by this call (the ones added since the last solve) */
   int32_t linear_solver;       /* PCG kernel the plan chose: 0 global block-Jacobi, 1 shared-memory block-Jacobi,
-                                * 3 two-level with 3 coarse modes, 6 two-level with 6 coarse modes; -1 no linear solve planned */
-  int32_t linear_solves;       /* PCG solves this call ran, retries at a larger regulariser included: one per iteration
-                                * under LM; under dogleg none for an iteration that reuses the Gauss-Newton step */
+                                * 3 two-level with 3 coarse modes, 6 two-level with 6 coarse modes; 8 block-sparse Cholesky
+                                * (linear_solver_type = 1, pcg_iterations stays 0); -1 no linear solve planned */
+  int32_t linear_solves;       /* PCG solves or Cholesky factorisations this call ran, retries at a larger regulariser
+                                * included: one per iteration under LM; under dogleg none for an iteration that reuses the
+                                * Gauss-Newton step. setup_ms includes the Cholesky analysis when one ran */
 } b200pg_summary;
 
 typedef struct b200pg b200pg;
@@ -295,6 +302,17 @@ int b200pg_solve(b200pg * h, b200pg_summary * summary_or_null);
 /* ScanSolver::GetCorrections (Mapper.h:988): all nodes after the last solve; returns count
  * written (<= cap). Empty after b200pg_clear(). */
 int32_t b200pg_get_corrections(const b200pg * h, int32_t * ids, double * poses, int32_t cap);
+/* The host analysis of the Cholesky linear solver, stateless and without a device: nodes 0..n-1, edges [e][2] node
+ * indices, fixed = the constant node or -1. The free nodes are the ones in some edge, except fixed. info = {free block
+ * columns, nonzero 3x3 blocks of L (diagonal included), supernodes, supernodal critical-path length, widest supernode
+ * (block columns), tallest panel (block rows), factor flops (sum over scalar columns of the squared column count), 0};
+ * order (may be NULL, else cap >= free nodes) receives the free nodes in elimination order. The ordering is a function of
+ * the free nodes and the set of adjacent pairs alone. A solve with linear_solver_type = 1 runs this same analysis. */
+int b200pg_cholesky_analyze(int32_t n, int32_t e, const int32_t * edge_nodes, int32_t fixed, int64_t info[8], int32_t * order,
+                            int32_t cap);
+/* The info record of the analysis the handle's last Cholesky solve used (zeros when there was none), with info[7] = the
+ * analyses this handle has run. */
+int b200pg_factor_info(const b200pg * h, int64_t info[8]);
 
 /* ------------------------------------------------------------------------------------------
  * Occupancy grid: karto::OccupancyGrid::CreateFromScans (Karto.h:5946-5961), the map-publish step

@@ -27,7 +27,8 @@ public:
   {
 #ifdef B200_WITH_ROS
     std::map<std::string, std::string> kv;
-    for (const char * k : {"ceres_linear_solver", "ceres_preconditioner", "ceres_trust_strategy", "ceres_dogleg_type", "ceres_loss_function"}) {
+    for (const char * k : {"ceres_linear_solver", "ceres_preconditioner", "ceres_trust_strategy", "ceres_dogleg_type", "ceres_loss_function",
+                           "b200_linear_solver"}) {
       std::string v;
       if (!node->has_parameter(k)) node->declare_parameter(k, std::string(""));
       if (node->get_parameter(k, v) && !v.empty()) kv[k] = v;
@@ -56,6 +57,10 @@ public:
       } else if (k == "ceres_trust_strategy") {   // :68-76
         if (v == "LEVENBERG_MARQUARDT") ++applied;
         else fprintf(stderr, "B200Solver: trust strategy '%s' is not available, using LEVENBERG_MARQUARDT\n", v.c_str());
+      } else if (k == "b200_linear_solver") {   // this library's own choice; ceres_linear_solver does not select it
+        if (v == "PCG") { o.linear_solver_type = 0; ++applied; }
+        else if (v == "SPARSE_NORMAL_CHOLESKY") { o.linear_solver_type = 1; ++applied; }
+        else fprintf(stderr, "B200Solver: unknown b200_linear_solver '%s', keeping the current linear solver\n", v.c_str());
       } else if (k == "ceres_linear_solver" || k == "ceres_preconditioner" || k == "ceres_dogleg_type") {
         ++applied;   // accepted: the linear solve is the library's block-sparse PCG whatever Ceres back end is named
       } else if (k == "max_num_iterations") { o.max_num_iterations = atoi(v.c_str()); ++applied; }
@@ -66,6 +71,15 @@ public:
     }
     if (b200pg_set_opts(h_, &o) != B200_OK) return -1;
     return applied;
+  }
+
+  // the options ConfigureFromStrings left on the handle
+  b200pg_opts GetOptions() const
+  {
+    std::lock_guard<std::mutex> lock(mu_);
+    b200pg_opts o;
+    b200pg_get_opts(h_, &o);
+    return o;
   }
 
   void Compute() override   // solvers/ceres_solver.cpp:214-269

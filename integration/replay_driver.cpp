@@ -68,6 +68,13 @@ int krep_solver_configure(void * rp, const char * key, const char * value)
   return r->solver->ConfigureFromStrings({{std::string(key), std::string(value)}});
 }
 
+// b200pg_opts.linear_solver_type of the adapter's handle (what b200_linear_solver selected), -1 without a solver
+int krep_solver_linear_solver_type(void * rp)
+{
+  Replay * r = static_cast<Replay *>(rp);
+  return r->solver ? r->solver->GetOptions().linear_solver_type : -1;
+}
+
 // Mapper::Reset (Mapper.cpp:2656-2677) deletes both scan matchers; krep_destroy deletes the mapper.  With the matcher shim
 // linked, b200_shim_live_handles() must drop to 0 afterwards (no leaked device state).
 void krep_reset_mapper(void * rp) { static_cast<Replay *>(rp)->mapper.Reset(); }

@@ -56,7 +56,7 @@ class PgOpts(C.Structure):
                 ("max_consecutive_nonmonotonic_steps", C.c_int32), ("max_num_consecutive_invalid_steps", C.c_int32),
                 ("pcg_tolerance", C.c_double), ("pcg_max_iterations", C.c_int32),
                 ("loss_function", C.c_int32), ("loss_scale", C.c_double),
-                ("trust_region_strategy", C.c_int32), ("dogleg_type", C.c_int32)]
+                ("trust_region_strategy", C.c_int32), ("dogleg_type", C.c_int32), ("linear_solver_type", C.c_int32)]
 
 
 class OgParams(C.Structure):
@@ -141,6 +141,8 @@ def lib():
         L.b200pg_num_edges.argtypes = [C.c_void_p]
         L.b200pg_solve.argtypes = [C.c_void_p, C.POINTER(PgSummary)]
         L.b200pg_get_corrections.argtypes = [C.c_void_p, _IP, _DP, C.c_int32]
+        L.b200pg_cholesky_analyze.argtypes = [C.c_int32, C.c_int32, _IP, C.c_int32, C.POINTER(C.c_int64), _IP, C.c_int32]
+        L.b200pg_factor_info.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     L.b200og_default_params.argtypes = [C.POINTER(OgParams)]
     L.b200og_create.argtypes = [C.POINTER(OgParams), C.POINTER(C.c_void_p)]
     L.b200og_destroy.argtypes = [C.c_void_p]
@@ -434,6 +436,21 @@ class ScanMatcher:
         return dict(valid_points=t[0] / n, raster=t[1] / n, lookup_tables=t[2] / n, volume=t[3] / n, epilogue=t[4] / n, matches=int(t[5]))
 
 
+FACTOR_INFO = ("columns", "nnz_blocks", "supernodes", "critical_path", "max_width", "max_rows", "flops", "analyses")
+
+
+def cholesky_analyze(n: int, edge_nodes, fixed: int = 0):
+    """b200pg_cholesky_analyze: the host analysis of the Cholesky linear solver for nodes 0..n-1 and edges [e, 2] of node
+    indices, `fixed` the constant node (-1 for none). Returns (info dict keyed by FACTOR_INFO, free nodes in elimination
+    order)."""
+    ed = np.ascontiguousarray(np.asarray(edge_nodes, dtype=np.int32).reshape(-1, 2))
+    info = np.zeros(8, dtype=np.int64)
+    order = np.zeros(max(n, 1), dtype=np.int32)
+    _check(lib().b200pg_cholesky_analyze(int(n), len(ed), _ip(ed), int(fixed), info.ctypes.data_as(C.POINTER(C.c_int64)),
+                                         _ip(order), max(n, 1)))
+    return dict(zip(FACTOR_INFO, (int(v) for v in info))), order[:int(info[0])].copy()
+
+
 class ScanSolver:
     """karto::ScanSolver (Mapper.h:954-1065) as implemented by solver_plugins::CeresSolver
     (solvers/ceres_solver.cpp), on the GPU."""
@@ -534,6 +551,13 @@ class ScanSolver:
         poses = np.zeros((max(n, 1), 3))
         m = lib().b200pg_get_corrections(self._h, _ip(ids), _dp(poses), n)
         return ids[:m], poses[:m]
+
+    def factor_info(self):
+        """b200pg_factor_info: the analysis the last Cholesky solve used (dict keyed by FACTOR_INFO; zeros before one),
+        with 'analyses' = the analyses this solver has run."""
+        info = np.zeros(8, dtype=np.int64)
+        _check(lib().b200pg_factor_info(self._h, info.ctypes.data_as(C.POINTER(C.c_int64))))
+        return dict(zip(FACTOR_INFO, (int(v) for v in info)))
 
     def num_nodes(self):
         return lib().b200pg_num_nodes(self._h)

@@ -1,5 +1,6 @@
 """Tiny workloads for compute-sanitizer (memcheck / racecheck / initcheck): a sweep of a few pairs through the fast and the
-generic kernel (with refine), a single match, and a small pose-graph solve."""
+generic kernel (with refine), a single match, a small pose-graph solve on the PCG kernels, and the same solve on the
+Cholesky linear solver ("pg_chol": supernodes with several updating descendants, under LM and dogleg)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -27,3 +28,13 @@ if which in ("all", "pg"):
     for nid, p in zip(g["ids"], g["init"]): s.AddNode(int(nid), p)
     for a, b, z, c in zip(g["edge_a"], g["edge_b"], g["z"], g["cov"]): s.AddConstraint(int(a), int(b), z, c)
     print("pg ok", s.Compute(), s.summary.pcg_iterations)
+if which in ("all", "pg_chol"):
+    g = synth.make_pose_graph(1, 200, 450, sigma_xy=0.03, sigma_th=0.01)
+    for strategy in (0, 1):
+        s = api.ScanSolver(max_num_iterations=3, linear_solver_type=1, trust_region_strategy=strategy)
+        for nid, p in zip(g["ids"], g["init"]): s.AddNode(int(nid), p)
+        for a, b, z, c in zip(g["edge_a"], g["edge_b"], g["z"], g["cov"]): s.AddConstraint(int(a), int(b), z, c)
+        ok = s.Compute()
+        info = s.factor_info()
+        assert s.summary.linear_solver == 8 and info["supernodes"] > 1 and info["critical_path"] > 2, info
+        print("pg_chol ok", strategy, ok, s.summary.linear_solves, info)
