@@ -260,7 +260,9 @@ typedef struct b200pg_summary {
   float wall_ms;               /* host wall time of the whole call                     */
   int32_t uploaded_edges;      /* constraints copied to the device by this call (the ones added since the last solve) */
   int32_t linear_solver;       /* PCG kernel the plan chose: 0 global block-Jacobi, 1 shared-memory block-Jacobi,
-                                * 3 two-level with 3 coarse modes, 6 two-level with 6 coarse modes; 8 block-sparse Cholesky
+                                * 3 two-level with 3 coarse modes, 6 two-level with 6 coarse modes, 13 / 16 the same
+                                * two-level preconditioner with 3 / 6 coarse modes on global-memory aggregates and a dense
+                                * coarse inverse (graphs too large for 3 / 6); 8 block-sparse Cholesky
                                 * (linear_solver_type = 1, pcg_iterations stays 0); -1 no linear solve planned */
   int32_t linear_solves;       /* PCG solves or Cholesky factorisations this call ran, retries at a larger regulariser
                                 * included: one per iteration under LM; under dogleg none for an iteration that reuses the

@@ -10,8 +10,9 @@
 //     strategies: LevenbergMarquardtStrategy (the default) or DoglegStrategy, traditional or subspace (DESIGN.md §4).
 //   * inner solve: instead of SPARSE_NORMAL_CHOLESKY, preconditioned CG on the 3x3-block normal equations inside ONE
 //     persistent cooperative kernel per solve, planned from the graph's rows: two-level (block Jacobi plus 6 or 3 coarse modes
-//     per aggregate, flag exchanges between CTAs; the default), block Jacobi with each CTA's rows in shared memory, or block
-//     Jacobi from global memory. Reductions are summed in a fixed order.  Opt-in (linear_solver_type = 1): the exact solve
+//     per aggregate, flag exchanges between CTAs; the default), the same two-level preconditioner on global-memory aggregates
+//     with a dense coarse inverse (graphs too large for shared memory), block Jacobi with each CTA's rows in shared memory, or
+//     block Jacobi from global memory. Reductions are summed in a fixed order.  Opt-in (linear_solver_type = 1): the exact solve
 //     SPARSE_NORMAL_CHOLESKY does, a supernodal FP64 Cholesky in one persistent cooperative kernel per solve (k_pg_cholesky)
 //     after a host symbolic analysis (cholesky_analyze).
 //   * one fused kernel evaluates every edge's residual, both Jacobian blocks (analytic) and the
@@ -272,15 +273,20 @@ __global__ void k_pg_reduce(PgDev d, int nparts, int slot_sum, int slot_max)
   if (slot_max >= 0) d.scalars[slot_max] = m;
 }
 
-// y_i = sum_j A_ij v_j for the scaled normal matrix plus damping: (Hd_i + D_i^2) v_i + sum_e M v_other
+__device__ __forceinline__ double ld_cg(const double * p) { return __ldcg(p); }
+
+// y_i = sum_j A_ij v_j for the scaled normal matrix plus damping: (Hd_i + D_i^2) v_i + sum_e M v_other.
+// kL2: read v0 / v1 through L2 (ld.global.cg), for vectors other CTAs of the same launch write between flag exchanges.
+template <bool kL2 = false>
 __device__ __forceinline__ void spmv_row(const PgDev & d, int i, const double * __restrict__ v0,
                                          const double * __restrict__ v1, double beta, double inv_radius, double out[3],
                                          double vi[3])
 {
   // effective vector v = v0 + beta * v1 (v1 may be null)
+  auto ldv = [](const double * p) { return kL2 ? ld_cg(p) : *p; };
   auto ld = [&](int j, double w[3]) {
-    w[0] = v0[3 * j]; w[1] = v0[3 * j + 1]; w[2] = v0[3 * j + 2];
-    if (v1) { w[0] += beta * v1[3 * j]; w[1] += beta * v1[3 * j + 1]; w[2] += beta * v1[3 * j + 2]; }
+    w[0] = ldv(v0 + 3 * j); w[1] = ldv(v0 + 3 * j + 1); w[2] = ldv(v0 + 3 * j + 2);
+    if (v1) { w[0] += beta * ldv(v1 + 3 * j); w[1] += beta * ldv(v1 + 3 * j + 1); w[2] += beta * ldv(v1 + 3 * j + 2); }
   };
   ld(i, vi);
   const double * h = d.Hd + 6 * i, * dg = d.diag + 3 * i;
@@ -345,8 +351,6 @@ __device__ __forceinline__ void jacobi_block(const PgDev & d, int i, double inv_
   const double id = 1.0 / (a00 * c00 + a01 * c01 + a02 * c02);
   mi[0] = c00 * id; mi[1] = c01 * id; mi[2] = c02 * id; mi[3] = c11 * id; mi[4] = c12 * id; mi[5] = c22 * id;
 }
-
-__device__ __forceinline__ double ld_cg(const double * p) { return __ldcg(p); }
 
 // The shared-memory kernels keep one CTA's rows [lo, hi) of the normal matrix: the off-diagonal blocks in CSR slot order
 // (sB, oriented for the row's node), each slot's neighbour (sCol) and the rows' starts (sStart); the CTA's vectors are
@@ -1109,6 +1113,440 @@ __global__ void __launch_bounds__(256, 2) k_pg_pcg_2lvl(PgDev d, Pcg2Cfg c, doub
 #undef PG_TICK
 }
 
+// ------------------------------------------------------------------------------------------
+// k_pg_pcg_2lvl_g: the preconditioner of k_pg_pcg_2lvl (same coarse modes, same flag exchanges, same coarse-residual
+// recurrence) for graphs whose aggregates do not fit shared memory (DESIGN.md §4 "Large graphs").
+//   * Aggregates are contiguous node ranges sized by the plan; CTA b owns aggregates [b apc, (b + 1) apc). The block rows,
+//     the preconditioner blocks (d.Minv) and the CG vectors stay in global memory (L2 up to a few tens of MB, HBM beyond).
+//   * Ac = P^T (H + D) P is assembled densely into global memory ([ld][ld], ld = CM na rounded up to kGjTile; the padding
+//     is the identity) from the same block formulas, one warp per aggregate adding its slots in CSR order. A grid-wide
+//     blocked Gauss-Jordan (kGjPanel columns per step, two grid barriers per step) inverts it in place once per solve.
+//   * Per CG iteration each CTA applies its CM apc rows of Ac^-1 to the coarse residual (a dense mat-vec spread over the
+//     grid), and P^T q travels through global memory (gPtq) ahead of the {p.q} flag, so the exchanges stay
+//     {p.q, P^T q} and {r.z, r.r}.
+// Every sum runs in a fixed order: results are bit-reproducible.
+// ------------------------------------------------------------------------------------------
+constexpr int kG2Threads = 512;
+constexpr int kGjPanel = 32;   // columns one Gauss-Jordan step eliminates (one per lane of a warp)
+constexpr int kGjTile = 64;    // the rank-kGjPanel update runs on kGjTile x kGjTile tiles
+struct Pcg2GCfg {
+  int na;                      // aggregates
+  int apc;                     // aggregates per CTA
+  int ld;                      // leading dimension of Ac: CM na rounded up to kGjTile
+  const int32_t * agg_start;   // [na + 1] contiguous node ranges
+  const int32_t * agg_of;      // [N]
+  double * gz;                 // [N][3]
+  double * gp;                 // [2][N][3]
+  double * gPt;                // [N][10] P~ base block of every node + its s (as Pcg2Cfg::gPt)
+  double * Ac;                 // [ld][ld] coarse matrix, then its inverse
+  double * Cb, * Tb;           // [kGjPanel][ld] a Gauss-Jordan step's old column panel and new row panel
+  double * gPtq;               // [ld] P^T q of the current iteration
+  double * grc;                // [ld] initial coarse residual P^T b
+  double * e1;                 // [2][G] slots: {p.q partial}
+  double * e2;                 // [2][G] slots: {r.z partial, r.r partial}
+  unsigned int * bar;          // atomic barrier counter (set-up only)
+};
+
+// In-place Gauss-Jordan inverse of a kGjPanel x kGjPanel block held by one warp, lane j holding column j (col[r] = D[r][j]).
+// A pivot that is zero or (numerically) dependent on the earlier ones has its row and column replaced by the identity's, as
+// in k_pg_pcg_2lvl's pivot blocks.
+__device__ __forceinline__ void gj_invert_cols(double (&col)[kGjPanel], int lane)
+{
+  double dself = 0;
+#pragma unroll
+  for (int r = 0; r < kGjPanel; ++r)
+    if (r == lane) dself = col[r];
+#pragma unroll
+  for (int p = 0; p < kGjPanel; ++p) {
+    const double d0 = fabs(__shfl_sync(0xffffffffu, dself, p));
+    double piv = __shfl_sync(0xffffffffu, col[p], p);
+    if (!(fabs(piv) > 1e-12 * d0) || !(d0 > 1e-300)) {   // warp-uniform
+      col[p] = 0.0;
+      if (lane == p) {
+#pragma unroll
+        for (int r = 0; r < kGjPanel; ++r) col[r] = 0.0;
+        col[p] = 1.0;
+      }
+      piv = 1.0;
+    }
+    const double inv = 1.0 / piv;
+    col[p] = lane == p ? inv : col[p] * inv;   // row p
+#pragma unroll
+    for (int r = 0; r < kGjPanel; ++r) {
+      if (r == p) continue;
+      const double cr = __shfl_sync(0xffffffffu, col[r], p);   // a[r][p] before this step
+      col[r] = lane == p ? -cr * inv : col[r] - cr * col[p];
+    }
+  }
+}
+
+template <int CM>
+__global__ void __launch_bounds__(kG2Threads, 1) k_pg_pcg_2lvl_g(PgDev d, Pcg2GCfg c, double inv_radius, double tol, int max_iter)
+{
+  static_assert(CM == 3 || CM == 6, "coarse modes per aggregate");
+  extern __shared__ __align__(16) unsigned char sm_raw[];
+  __shared__ double red[CM * 32];
+  __shared__ double bc[1];
+  __shared__ double s_small[2];
+  const int T = blockDim.x, tid = threadIdx.x, G = gridDim.x, I = blockIdx.x;
+  const int lane = tid & 31, warp = tid >> 5, nwarps = T >> 5;
+  const int nc = CM * c.na, ld = c.ld;
+  const int a_lo = min(c.na, I * c.apc), a_hi = min(c.na, a_lo + c.apc);
+  const int lo = c.agg_start[a_lo], hi = c.agg_start[a_hi];
+  double * sRc = reinterpret_cast<double *>(sm_raw);   // [ld] coarse residual (identical in all CTAs)
+  double * sW = sRc + ld;   // scratch: assembly staging, then the Gauss-Jordan tiles, then the exchange and CM apc coarse values
+  unsigned int bar_target = 0;
+  const double SENT = pg_sentinel();
+  unsigned long long t_start = 0, t_setup = 0, t_gj = 0;
+  if (I == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
+
+  // P^T v of every own aggregate into out[CM a + m]: the whole CTA on one aggregate at a time, threads over its nodes, then
+  // a fixed-order block reduction (every thread calls it)
+  auto aggregate_pt = [&](const double * v, double * out) {
+    for (int a = a_lo; a < a_hi; ++a) {
+      double u[CM];
+#pragma unroll
+      for (int m = 0; m < CM; ++m) u[m] = 0.0;
+      for (int i = c.agg_start[a] + tid; i < c.agg_start[a + 1]; i += T) {
+        const double * pt = c.gPt + 10 * (size_t)i;
+        const double v0 = v[3 * i], v1 = v[3 * i + 1], v2 = v[3 * i + 2];
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+          const double w = pt[q] * v0 + pt[3 + q] * v1 + pt[6 + q] * v2;
+          u[q] += w;
+          if constexpr (CM > 3) u[3 + q] += pt[9] * w;
+        }
+      }
+      block_sum<CM>(u, red);
+      if (tid == 0)
+#pragma unroll
+        for (int m = 0; m < CM; ++m) out[CM * a + m] = u[m];
+    }
+  };
+
+  // ---- set-up 1: Ac = 0 (identity on the padding); per own node Minv, P~ and s, r = b, y = 0, p = 0; empty slots ----
+  for (size_t k = (size_t)I * T + tid; k < (size_t)ld * ld; k += (size_t)G * T) {
+    const size_t r = k / ld;
+    c.Ac[k] = (r >= (size_t)nc && k == r * ld + r) ? 1.0 : 0.0;
+  }
+  for (int a = a_lo + warp; a < a_hi; a += nwarps) {
+    const int alo = c.agg_start[a], nloc = c.agg_start[a + 1] - alo;
+    double cx = 0, cy = 0, cnt = 0;   // centroid of the aggregate's free nodes
+    for (int n = lane; n < nloc; n += 32)
+      if (d.is_free[alo + n]) { cx += d.x[3 * (alo + n)]; cy += d.x[3 * (alo + n) + 1]; cnt += 1.0; }
+    cx = warp_sum(cx); cy = warp_sum(cy); cnt = warp_sum(cnt);
+    if (cnt > 0) { cx /= cnt; cy /= cnt; }
+    for (int n = lane; n < nloc; n += 32) {
+      const int i = alo + n;
+      double hb[6];
+      jacobi_block(d, i, inv_radius, hb, d.Minv + 6 * i);
+      double * pt = c.gPt + 10 * (size_t)i;
+      const double f = d.is_free[i] ? 1.0 : 0.0;
+      const double isx = f / d.scale[3 * i], isy = f / d.scale[3 * i + 1], ist = f / d.scale[3 * i + 2];
+      pt[0] = isx; pt[1] = 0;   pt[2] = -(d.x[3 * i + 1] - cy) * isx;
+      pt[3] = 0;   pt[4] = isy; pt[5] = (d.x[3 * i] - cx) * isy;
+      pt[6] = 0;   pt[7] = 0;   pt[8] = ist;
+      pt[9] = (CM > 3 && nloc > 1 && cnt >= 2.0) ? 2.0 * n / (double)(nloc - 1) - 1.0 : 0.0;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        d.pr[3 * i + k] = d.g[3 * i + k]; d.y[3 * i + k] = 0.0; c.gp[3 * i + k] = 0.0;
+      }
+    }
+  }
+  if (tid < 2) c.e1[((size_t)tid * G + I) * kSlotStride] = SENT;
+  if (tid < 4) c.e2[((size_t)(tid >> 1) * G + I) * kSlotStride + (tid & 1)] = SENT;
+  bar_target += G;
+  grid_barrier(c.bar, bar_target);   // gPt, zeroed Ac and empty slots visible everywhere
+
+  // ---- set-up 2: rows CM a .. CM a + CM - 1 of Ac, a warp per own aggregate. Its items (the CSR slots of its nodes, then
+  // the nodes' diagonal blocks) are staged 32 at a time; lane l owns entries l and l + 32 of the CM x CM block and adds
+  // the staged items in order, flushing to Ac whenever the column block changes ----
+  {
+    double * stg = sW + (size_t)warp * 32 * 12;   // [32][12]: w3 = pi^T A_ij pj (9), s_i, s_j, column block
+    for (int a = a_lo + warp; a < a_hi; a += nwarps) {
+      const int alo = c.agg_start[a], ahi = c.agg_start[a + 1];
+      const int s_lo = d.adj_start[alo], nslots = d.adj_start[ahi] - s_lo, nitems = nslots + (ahi - alo);
+      double acc[2] = {0.0, 0.0};
+      int cur = -1;
+      auto flush = [&]() {
+        if (cur >= 0)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int e = lane + 32 * h;
+            if (e < CM * CM) c.Ac[(size_t)(CM * a + e / CM) * ld + CM * cur + e % CM] += acc[h];
+          }
+        acc[0] = 0.0; acc[1] = 0.0;
+      };
+      for (int t0 = 0; t0 < nitems; t0 += 32) {
+        const int t = t0 + lane;
+        if (t < nitems) {
+          double B[9], pj[9], sj;
+          int i, ct;
+          if (t < nslots) {
+            const int s = s_lo + t;
+            int l = alo, u = ahi - 1;   // the slot's node: the last i with adj_start[i] <= s
+            while (l < u) { const int m = (l + u + 1) >> 1; if (d.adj_start[m] <= s) l = m; else u = m - 1; }
+            i = l;
+            const int av = d.adj[s], e = av >> 1, side = av & 1;
+            const double * M = d.lin + (size_t)kLin * e + 21;
+            const int j = d.eidx[2 * e + (side ? 0 : 1)];
+#pragma unroll
+            for (int r = 0; r < 3; ++r)
+#pragma unroll
+              for (int q = 0; q < 3; ++q) B[3 * r + q] = side == 0 ? M[3 * r + q] : M[3 * q + r];
+#pragma unroll
+            for (int k = 0; k < 9; ++k) pj[k] = ld_cg(c.gPt + 10 * (size_t)j + k);
+            sj = ld_cg(c.gPt + 10 * (size_t)j + 9);
+            ct = c.agg_of[j];
+          } else {
+            i = alo + (t - nslots);
+            double hb[6], mi[6];
+            jacobi_block(d, i, inv_radius, hb, mi);
+            B[0] = hb[0]; B[1] = hb[1]; B[2] = hb[2]; B[3] = hb[1]; B[4] = hb[3]; B[5] = hb[4];
+            B[6] = hb[2]; B[7] = hb[4]; B[8] = hb[5];
+#pragma unroll
+            for (int k = 0; k < 9; ++k) pj[k] = ld_cg(c.gPt + 10 * (size_t)i + k);
+            sj = ld_cg(c.gPt + 10 * (size_t)i + 9);
+            ct = a;
+          }
+          double pi[9], w[9];
+#pragma unroll
+          for (int k = 0; k < 9; ++k) pi[k] = ld_cg(c.gPt + 10 * (size_t)i + k);
+          const double si = ld_cg(c.gPt + 10 * (size_t)i + 9);
+#pragma unroll
+          for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int q = 0; q < 3; ++q) w[3 * r + q] = B[3 * r] * pj[q] + B[3 * r + 1] * pj[3 + q] + B[3 * r + 2] * pj[6 + q];
+          double * o = stg + 12 * lane;
+#pragma unroll
+          for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int q = 0; q < 3; ++q) o[3 * r + q] = pi[r] * w[q] + pi[3 + r] * w[3 + q] + pi[6 + r] * w[6 + q];
+          o[9] = si; o[10] = sj; o[11] = (double)ct;
+        }
+        __syncwarp();
+        const int nt = min(32, nitems - t0);
+        for (int u = 0; u < nt; ++u) {
+          const double * o = stg + 12 * u;
+          const int ct = (int)o[11];
+          if (ct != cur) { flush(); cur = ct; }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int e = lane + 32 * h;
+            if (e < CM * CM) {
+              const int R = e / CM, Q = e % CM;
+              double v = o[3 * (R % 3) + Q % 3];
+              if (R >= 3) v *= o[9];
+              if (Q >= 3) v *= o[10];
+              acc[h] += v;
+            }
+          }
+        }
+        __syncwarp();
+      }
+      flush();
+      __syncwarp();
+      // a mode without a free node (or the s-modes of an aggregate with fewer than two) has a zero row and column: identity
+      if (lane < CM) {
+        double * dg = c.Ac + (size_t)(CM * a + lane) * ld + CM * a + lane;
+        if (*dg == 0.0) *dg = 1.0;
+      }
+    }
+  }
+  bar_target += G;
+  grid_barrier(c.bar, bar_target);
+  if (I == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_setup));
+
+  // ---- set-up 3: in-place blocked Gauss-Jordan. Step K (columns k0 .. k0 + 31): D = A(K, K);
+  //   T = D^-1 [A(K, :) with the identity in columns K]   (the new rows K),
+  //   C = A(:, K) with -I in rows K                        (the old columns K),
+  //   A(i, j) <- [i, j outside K] A(i, j) - sum_k C(i, k) T(k, j)   for every (i, j),
+  // which leaves D^-1, D^-1 A(K, :), -A(:, K) D^-1 and the Schur complement in place; after the last step A = Ac^-1 ----
+  {
+    double * sC = sW, * sT = sW + kGjPanel * kGjTile, * sD = sT + kGjPanel * kGjTile;   // [32][64], [32][64], [32][32]
+    const int ntile = ld / kGjTile;
+    for (int k0 = 0; k0 < ld; k0 += kGjPanel) {
+      if (warp == 0) {   // every CTA inverts the pivot block the same way
+        double col[kGjPanel];
+#pragma unroll
+        for (int r = 0; r < kGjPanel; ++r) col[r] = ld_cg(c.Ac + (size_t)(k0 + r) * ld + k0 + lane);
+        gj_invert_cols(col, lane);
+#pragma unroll
+        for (int r = 0; r < kGjPanel; ++r) sD[r * kGjPanel + lane] = col[r];
+      }
+      __syncthreads();
+      for (int j = I * T + tid; j < ld; j += G * T) {
+        const bool piv = j >= k0 && j < k0 + kGjPanel;
+        double v[kGjPanel];
+#pragma unroll
+        for (int m = 0; m < kGjPanel; ++m) v[m] = piv ? (j - k0 == m ? 1.0 : 0.0) : ld_cg(c.Ac + (size_t)(k0 + m) * ld + j);
+#pragma unroll 4
+        for (int k = 0; k < kGjPanel; ++k) {
+          double t = 0;
+#pragma unroll
+          for (int m = 0; m < kGjPanel; ++m) t += sD[k * kGjPanel + m] * v[m];
+          c.Tb[(size_t)k * ld + j] = t;
+        }
+#pragma unroll
+        for (int k = 0; k < kGjPanel; ++k) c.Cb[(size_t)k * ld + j] = piv ? (j - k0 == k ? -1.0 : 0.0) : ld_cg(c.Ac + (size_t)j * ld + k0 + k);
+      }
+      bar_target += G;
+      grid_barrier(c.bar, bar_target);
+      for (int tl = I; tl < ntile * ntile; tl += G) {
+        const int i0 = (tl / ntile) * kGjTile, j0 = (tl % ntile) * kGjTile;
+        for (int k = tid; k < kGjPanel * kGjTile; k += T) {
+          const int kk = k / kGjTile, x = k % kGjTile;
+          sC[k] = ld_cg(c.Cb + (size_t)kk * ld + i0 + x);
+          sT[k] = ld_cg(c.Tb + (size_t)kk * ld + j0 + x);
+        }
+        __syncthreads();
+        const int r = tid >> 3, cl = tid & 7;   // row r of the tile, its columns cl + 8 m
+        const int i = i0 + r;
+        const bool rowK = i >= k0 && i < k0 + kGjPanel;
+        double o[8];
+#pragma unroll
+        for (int m = 0; m < 8; ++m) {
+          const int j = j0 + cl + 8 * m;
+          o[m] = (rowK || (j >= k0 && j < k0 + kGjPanel)) ? 0.0 : ld_cg(c.Ac + (size_t)i * ld + j);
+        }
+#pragma unroll 8
+        for (int k = 0; k < kGjPanel; ++k) {
+          const double cv = sC[k * kGjTile + r];
+#pragma unroll
+          for (int m = 0; m < 8; ++m) o[m] -= cv * sT[k * kGjTile + cl + 8 * m];
+        }
+#pragma unroll
+        for (int m = 0; m < 8; ++m) c.Ac[(size_t)i * ld + j0 + cl + 8 * m] = o[m];
+        __syncthreads();
+      }
+      bar_target += G;
+      grid_barrier(c.bar, bar_target);
+    }
+  }
+  if (I == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_gj));
+
+  // ---- CG start: coarse residual P^T b (every CTA keeps all of it), z = M^-1 r ----
+  double * sEx = sW;                       // [2 G] polled exchange values
+  double * sYc = sW + 2 * (size_t)G;       // [CM apc] Ac^-1 rc on the own aggregates
+  double accb[1] = {0};
+  for (int k = 3 * lo + tid; k < 3 * hi; k += T) accb[0] += d.g[k] * d.g[k];
+  aggregate_pt(d.g, c.grc);
+  block_sum<1>(accb, red);
+  if (tid == 0) d.partial[I] = accb[0];
+  bar_target += G;
+  grid_barrier(c.bar, bar_target);
+  const double bb = grid_total(d, 0, G, bc);
+  for (int k = tid; k < ld; k += T) sRc[k] = k < nc ? ld_cg(c.grc + k) : 0.0;
+  __syncthreads();
+
+  // z = blockJacobi^-1 r + P Ac^-1 rc on the own nodes (published to gz); partial r.z and r.r through a2
+  auto apply_precond = [&](double (&a2)[2]) {
+    for (int row = warp; row < CM * (a_hi - a_lo); row += nwarps) {   // a warp per row of Ac^-1
+      const double * Ai = c.Ac + (size_t)(CM * a_lo + row) * ld;
+      double a = 0;
+      for (int j = lane; j < nc; j += 32) a += ld_cg(Ai + j) * sRc[j];
+      a = warp_sum(a);
+      if (lane == 0) sYc[row] = a;
+    }
+    __syncthreads();
+    a2[0] = 0; a2[1] = 0;
+    for (int k = 3 * lo + tid; k < 3 * hi; k += T) {
+      const int i = k / 3, r = k - 3 * i;
+      const double * pt = c.gPt + 10 * (size_t)i;
+      const double * yc = sYc + CM * (c.agg_of[i] - a_lo);
+      const double r0 = d.pr[3 * i], r1 = d.pr[3 * i + 1], r2 = d.pr[3 * i + 2];
+      double z = sym3_row(d.Minv + 6 * i, r, r0, r1, r2);
+      double y0 = yc[0], y1 = yc[1], y2 = yc[2];
+      if constexpr (CM > 3) { const double sn = pt[9]; y0 += sn * yc[3]; y1 += sn * yc[4]; y2 += sn * yc[5]; }
+      z += pt[3 * r] * y0 + pt[3 * r + 1] * y1 + pt[3 * r + 2] * y2;
+      c.gz[k] = z;
+      const double rk = d.pr[k];
+      a2[0] += rk * z;
+      a2[1] += rk * rk;
+    }
+  };
+  double a2[2];
+  apply_precond(a2);
+  block_sum<2>(a2, red);
+  if (tid == 0) d.partial[kMaxPartials + I] = a2[0];
+  bar_target += G;
+  grid_barrier(c.bar, bar_target);
+  double rz = grid_total(d, 1, G, bc);
+  double rr = bb;
+  const double stop = tol * tol * bb;
+  int it = 0;
+  double beta = 0.0;
+  int cur = 0;
+  if (bb > 0.0) {
+    while (it < max_iter) {
+      const int par = it & 1;
+      const double * gpo = c.gp + (size_t)cur * 3 * d.N;
+      double * gpn = c.gp + (size_t)(cur ^ 1) * 3 * d.N;
+      double * e1 = c.e1 + (size_t)par * G * kSlotStride, * e2 = c.e2 + (size_t)par * G * kSlotStride;
+      // ---- phase A: p_new = z + beta p_old ; q = A p_new ; p.q ; P^T q of the own aggregates ----
+      double a1[1] = {0};
+      for (int i = lo + tid; i < hi; i += T) {
+        double q[3], pv[3];
+        spmv_row<true>(d, i, c.gz, gpo, beta, inv_radius, q, pv);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { gpn[3 * i + k] = pv[k]; d.pq[3 * i + k] = q[k]; }
+        a1[0] += pv[0] * q[0] + pv[1] * q[1] + pv[2] * q[2];
+      }
+      block_sum<1>(a1, red);
+      __syncthreads();
+      aggregate_pt(d.pq, c.gPtq);
+      __syncthreads();
+      if (tid == 0) {
+        __threadfence();   // p_new and P^T q of this CTA visible before the flagged value
+        e1[(size_t)I * kSlotStride] = a1[0];
+      }
+      poll_slots<1>(e1, G, sEx);
+      // every CTA published E1(it) only after it finished reading E2(it-1): those slots can be recycled now
+      if (it > 0 && tid < 2) c.e2[((size_t)(par ^ 1) * G + I) * kSlotStride + tid] = SENT;
+      const double pq = ordered_sum(sEx, G, 1, 0, bc);
+      const double alpha = rz / pq;
+      // ---- phase B: rc -= alpha P^T q ; y += alpha p ; r -= alpha q ; z = M^-1 r ----
+      for (int k = tid; k < nc; k += T) sRc[k] -= alpha * ld_cg(c.gPtq + k);
+      for (int k = 3 * lo + tid; k < 3 * hi; k += T) { d.y[k] += alpha * gpn[k]; d.pr[k] -= alpha * d.pq[k]; }
+      __syncthreads();
+      apply_precond(a2);
+      block_sum<2>(a2, red);
+      __syncthreads();
+      if (tid == 0) {
+        __threadfence();   // z of this CTA visible before the flagged values
+        double * m = e2 + (size_t)I * kSlotStride;
+        m[0] = a2[0]; m[1] = a2[1];
+      }
+      poll_slots<2>(e2, G, sEx);
+      // every CTA published E2(it) only after it finished reading E1(it) and gPtq(it): recycle own E1(it) slot
+      if (tid == 0) c.e1[((size_t)par * G + I) * kSlotStride] = SENT;
+      if (tid < 32) {
+        double u = 0, w = 0;
+        for (int k = tid; k < G; k += 32) { u += sEx[2 * k]; w += sEx[2 * k + 1]; }
+        u = warp_sum(u); w = warp_sum(w);
+        if (tid == 0) { s_small[0] = u; s_small[1] = w; }
+      }
+      __syncthreads();
+      const double rz_new = s_small[0];
+      rr = s_small[1];
+      ++it;
+      cur ^= 1;
+      if (!(rr > stop) || !(pq > 0.0)) break;
+      beta = rz_new / rz;
+      rz = rz_new;
+    }
+  }
+  if (I == 0 && tid == 0) {
+    unsigned long long t_end;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
+    d.scalars[8] = (double)it;
+    d.scalars[9] = bb > 0.0 ? sqrt(rr / bb) : 0.0;
+    d.scalars[10] = (double)(t_setup - t_start);   // ns: Minv, P~, Ac assembly
+    d.scalars[11] = (double)(t_gj - t_setup);      // ns: blocked Gauss-Jordan
+    d.scalars[12] = (double)(t_end - t_gj);        // ns: CG iterations
+  }
+}
+
 // candidate point: delta = -(y * scale) ; xc = x (+) delta on free nodes; partial ||x - xc||^2
 __global__ void __launch_bounds__(kPgThreads) k_pg_apply_step(PgDev d)
 {
@@ -1569,6 +2007,8 @@ struct b200pg {
   int coarse_modes = 6;   // two-level: coarse modes per aggregate (6 = rigid + linear deformation, 3 = rigid only)
   DevBuf<unsigned int> d_bar;
   bool force_global_pcg = false;
+  bool force_2lvl_global = false;   // B200PG_FORCE_2LVL_GLOBAL: plan k_pg_pcg_2lvl_g at any size
+  DevBuf<double> d_gAc, d_gCb, d_gTb, d_gPtq;   // k_pg_pcg_2lvl_g: dense coarse matrix / inverse and its step panels
   DevBuf<double> d_z, d_U, d_x, d_xc, d_scale, d_lin, d_Hd, d_g, d_diag, d_y, d_pr, d_pz, d_pp0, d_pp1, d_pq, d_Minv,
     d_partial, d_scalars;
   DevBuf<double> d_ygn;   // dogleg: the Gauss-Newton solution, kept for the iterations that reuse it
@@ -1805,7 +2245,8 @@ static void subspace_step(const DoglegModel & m, double radius, double & ca, dou
 }
 
 // The linear-solve kernel of a solve and how it is launched. kernel is the b200pg_summary.linear_solver code: 0 global
-// block-Jacobi, 1 shared-memory block-Jacobi, 3 / 6 two-level with that many coarse modes per aggregate (PCG), 8 Cholesky.
+// block-Jacobi, 1 shared-memory block-Jacobi, 3 / 6 two-level with that many coarse modes per aggregate (PCG), 13 / 16 the
+// same two-level preconditioner with global-memory aggregates and a dense coarse inverse (k_pg_pcg_2lvl_g), 8 Cholesky.
 constexpr int kLinearSolverCholesky = 8;
 struct PcgPlan {
   int kernel = 0;
@@ -1813,7 +2254,84 @@ struct PcgPlan {
   size_t smem_bytes = 0;    // dynamic shared memory
   PcgSmemCfg smem{};        // kernel 1
   Pcg2Cfg two_level{};      // kernels 3 and 6
+  Pcg2GCfg two_level_g{};   // kernels 13 and 16
 };
+
+constexpr int kMin2lvlGlobalNodes = 8192;
+constexpr int kMaxCoarse2lvlGlobal = 4096;
+
+// Algorithmic bytes of one CG iteration's fine level (SpMV, block-Jacobi, vector updates) on a graph of N nodes and `slots`
+// CSR slots (2 E): per node Hd, D, Minv and the ten vector streams (30 doubles), per slot its 3x3 block, the neighbour's
+// z and p and the slot's index words.
+static double pcg_fine_bytes(double N, double slots) { return 240.0 * N + 128.0 * slots; }
+
+// The coarse size of k_pg_pcg_2lvl_g: nc = CM x aggregates, with the dense Ac^-1 mat-vec (8 nc^2 bytes per iteration) held
+// to a quarter of the fine level's bytes, nc <= sqrt(fine / 32), at most kMaxCoarse2lvlGlobal (the inverse costs 2 nc^3 flops
+// and 16 nc^2 bytes per kGjPanel columns once per solve) and aggregates of at least 16 nodes.
+static int coarse_aggregates_2lvl_global(int N, int slots, int cm)
+{
+  const int nc = std::min(kMaxCoarse2lvlGlobal, (int)std::sqrt(pcg_fine_bytes(N, slots) / 32.0));
+  return std::max(1, std::min((N + 15) / 16, nc / cm));
+}
+
+// Plans k_pg_pcg_2lvl_g into P (kernel 13 or 16) when its dense coarse inverse fits the free device memory; otherwise
+// leaves P as it is (B200PG_DEBUG says why).
+static void plan_pcg_2lvl_global(b200pg * h, const std::vector<int32_t> & adj_start, int sms, cudaStream_t st, PcgPlan & P)
+{
+  const int N = (int)adj_start.size() - 1;
+  const int cm = h->coarse_modes >= 6 ? 6 : 3;
+  const int want = coarse_aggregates_2lvl_global(N, adj_start[N], cm);
+  std::vector<int32_t> agg_start, agg_of(N, 0);
+  const int per = (N + want - 1) / want;
+  for (int i = 0; i < N; i += per) agg_start.push_back(i);
+  agg_start.push_back(N);
+  const int na = (int)agg_start.size() - 1;
+  for (int a = 0; a < na; ++a)
+    for (int i = agg_start[a]; i < agg_start[a + 1]; ++i) agg_of[i] = a;
+  const int nc = cm * na, ld = (nc + kGjTile - 1) / kGjTile * kGjTile;
+  const void * fn = cm == 6 ? (const void *)k_pg_pcg_2lvl_g<6> : (const void *)k_pg_pcg_2lvl_g<3>;
+  // shared memory: the coarse residual, then the largest scratch of the three stages (assembly staging, Gauss-Jordan
+  // tiles, exchange + coarse values; the last is at most 2 G + cm na doubles, G <= 2 sms)
+  const size_t scratch = std::max<size_t>({(size_t)(kG2Threads / 32) * 32 * 12, 2 * kGjPanel * kGjTile + kGjPanel * kGjPanel,
+                                           4 * (size_t)sms + (size_t)nc});
+  const size_t bytes = ((size_t)ld + scratch) * sizeof(double);
+  int occ = 0;
+  if (bytes <= 220 * 1024) {
+    B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kG2Threads, bytes));
+    occ = std::min(occ, 2);
+  }
+  if (occ < 1) {
+    if (h->debug) fprintf(stderr, "[b200pg] two-level global plan: %zu B of shared memory for nc = %d do not fit; kernel 0\n", bytes, nc);
+    return;
+  }
+  const int apc = (na + std::min(na, occ * sms) - 1) / std::min(na, occ * sms);
+  const int G = (na + apc - 1) / apc;
+  // device memory the plan adds: Ac, the two step panels, P^T q and the initial coarse residual, P~, p and z, slots, indices
+  auto grow = [](const DevBuf<double> & b, size_t n) { return n > b.cap ? (n + n / 4 + 16) * sizeof(double) : (size_t)0; };
+  const size_t n3 = 3 * (size_t)N;
+  const size_t need = grow(h->d_gAc, (size_t)ld * ld) + grow(h->d_gCb, (size_t)kGjPanel * ld) + grow(h->d_gTb, (size_t)kGjPanel * ld) +
+                      grow(h->d_gPtq, ld) + grow(h->d_grc, ld) + grow(h->d_gPt, 10 * (size_t)N) + grow(h->d_gz, n3) + grow(h->d_gp, 2 * n3) +
+                      (size_t)(2 * N + na) * sizeof(int32_t) + 4 * (size_t)G * kSlotStride * sizeof(double);
+  size_t free_b = 0, total_b = 0;
+  B200_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  if (need + (size_t)64 * 1024 * 1024 > free_b) {
+    if (h->debug) fprintf(stderr, "[b200pg] two-level global plan: the dense coarse inverse (nc = %d, %zu MB) needs %zu MB, %zu MB free; kernel 0\n", nc, (size_t)ld * ld * 8 >> 20, need >> 20, free_b >> 20);
+    return;
+  }
+  if (h->debug) fprintf(stderr, "[b200pg] two-level global plan: %d aggregates x %d modes (nc = %d, ld = %d), %d nodes each, %d CTAs x %d aggregates, %zu B smem\n", na, cm, nc, ld, per, G, apc, bytes);
+  h->d_gAc.reserve((size_t)ld * ld); h->d_gCb.reserve((size_t)kGjPanel * ld); h->d_gTb.reserve((size_t)kGjPanel * ld);
+  h->d_gPtq.reserve(ld); h->d_grc.reserve(ld); h->d_gPt.reserve(10 * (size_t)N); h->d_gz.reserve(n3); h->d_gp.reserve(2 * n3);
+  h->d_bar.reserve(4096); h->d_e1.reserve((size_t)2 * G * kSlotStride); h->d_e2.reserve((size_t)2 * G * kSlotStride);
+  h->agg_start_h.swap(agg_start); h->agg_of_h.swap(agg_of);   // the vectors live in the handle
+  up(h->d_agg_start, h->agg_start_h, st); up(h->d_agg_of, h->agg_of_h, st);
+  P = PcgPlan{};
+  P.kernel = 10 + cm; P.blocks = G; P.smem_bytes = bytes;
+  Pcg2GCfg & c = P.two_level_g;
+  c.na = na; c.apc = apc; c.ld = ld; c.agg_start = h->d_agg_start.p; c.agg_of = h->d_agg_of.p;
+  c.gz = h->d_gz.p; c.gp = h->d_gp.p; c.gPt = h->d_gPt.p; c.Ac = h->d_gAc.p; c.Cb = h->d_gCb.p; c.Tb = h->d_gTb.p;
+  c.gPtq = h->d_gPtq.p; c.grc = h->d_grc.p; c.e1 = h->d_e1.p; c.e2 = h->d_e2.p; c.bar = h->d_bar.p;
+}
 
 // Picks the PCG kernel from the graph's CSR rows: shared-memory block-Jacobi where every CTA's rows fit, then the two-level
 // kernel where its aggregates fit (B200PG_PRECOND, B200PG_COARSE_MODES and B200PG_FORCE_GLOBAL_PCG narrow the choice).
@@ -1905,6 +2423,12 @@ static PcgPlan plan_pcg(b200pg * h, const std::vector<int32_t> & adj_start, cuda
       c2.grc = h->d_grc.p; c2.e1 = h->d_e1.p; c2.e2 = h->d_e2.p; c2.bar = h->d_bar.p; c2.gjflag = h->d_bar.p + 1;
     }
   }
+  // Past the shared-memory kernels' reach, the two-level preconditioner with global-memory aggregates instead of kernel 0.
+  // Below kMin2lvlGlobalNodes a plan ends on kernel 0 only when one row (a hub node) is too long for shared memory. Those
+  // graphs keep kernel 0 so that the plan of every graph of that size stays what it was before this kernel existed; which
+  // of the two kernels is faster there has not been measured. B200PG_FORCE_2LVL_GLOBAL plans it at any size.
+  if (h->precond == 1 && !h->force_global_pcg && (h->force_2lvl_global || (P.kernel == 0 && N >= kMin2lvlGlobalNodes)))
+    plan_pcg_2lvl_global(h, adj_start, sms, st, P);
   return P;
 }
 
@@ -2311,6 +2835,10 @@ struct Launcher {
       c.L = h->d_ch_L.p; c.z = h->d_ch_z.p; c.flag = h->d_ch_flag.p; c.ctl = h->d_ch_ctl.p; c.epoch = h->chol_epoch;
       void * args[] = {&d, &c, &shift};
       B200_CUDA(cudaLaunchCooperativeKernel((void *)k_pg_cholesky, dim3(plan.blocks), dim3(kCholThreads), args, 0, st));
+    } else if (plan.kernel == 13 || plan.kernel == 16) {
+      B200_CUDA(cudaMemsetAsync(h->d_bar.p, 0, sizeof(unsigned int), st));
+      void * args[] = {&d, &plan.two_level_g, &shift, &tol, &max_iter};
+      B200_CUDA(cudaLaunchCooperativeKernel(plan.kernel == 16 ? (void *)k_pg_pcg_2lvl_g<6> : (void *)k_pg_pcg_2lvl_g<3>, dim3(plan.blocks), dim3(kG2Threads), args, plan.smem_bytes, st));
     } else if (plan.kernel >= 3) {
       B200_CUDA(cudaMemsetAsync(h->d_bar.p, 0, (size_t)(plan.blocks + 1) * sizeof(unsigned int), st));
       void * args[] = {&d, &plan.two_level, &shift, &tol, &max_iter};
@@ -2368,6 +2896,9 @@ struct LmStrategy {
     if (L.h->debug && L.plan.kernel == kLinearSolverCholesky)
       fprintf(stderr, "[b200pg] lm %d: cholesky factor+forward %.1f us, backward %.1f us, residual %.1f us\n", it, sc[10] * 1e-3,
               sc[11] * 1e-3, sc[12] * 1e-3);
+    if (L.h->debug && (L.plan.kernel == 13 || L.plan.kernel == 16))
+      fprintf(stderr, "[b200pg] lm %d: pcg %d it, setup %.1f us, gauss-jordan %.1f us, cg %.1f us (%.2f us/it)\n", it, (int)sc[8],
+              sc[10] * 1e-3, sc[11] * 1e-3, sc[12] * 1e-3, sc[12] * 1e-3 / std::max(1.0, sc[8]));
     if (L.h->debug && (L.plan.kernel == 3 || L.plan.kernel == 6))
       fprintf(stderr, "[b200pg] lm %d: pcg %d it, setup %.1f us, gauss-jordan %.1f us, cg %.1f us (%.2f us/it: gather %.2f spmv+reduce %.2f exch1 %.2f precond %.2f exch2 %.2f)\n", it, (int)sc[8],
               sc[10] * 1e-3, sc[11] * 1e-3, sc[12] * 1e-3, sc[12] * 1e-3 / std::max(1.0, sc[8]), sc[13] * 1e-3 / std::max(1.0, sc[8]),
@@ -2654,6 +3185,7 @@ int b200pg_create(const b200pg_opts * opts, b200pg ** out)
   }
   require_device();
   if (const char * e = getenv("B200PG_FORCE_GLOBAL_PCG")) h->force_global_pcg = atoi(e) != 0;
+  if (const char * e = getenv("B200PG_FORCE_2LVL_GLOBAL")) h->force_2lvl_global = atoi(e) != 0;
   if (const char * e = getenv("B200PG_DEBUG")) h->debug = atoi(e) != 0;
   if (const char * e = getenv("B200PG_PRECOND")) h->precond = std::string(e) == "jacobi" ? 0 : 1;
   if (const char * e = getenv("B200PG_COARSE_MODES")) h->coarse_modes = atoi(e) >= 6 ? 6 : 3;

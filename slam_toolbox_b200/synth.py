@@ -322,6 +322,66 @@ def make_pose_graph(seed: int, n_nodes: int = 10000, n_edges: int = 40000, latti
     return dict(ids=ids, init=init, truth=truth, edge_a=ea, edge_b=eb, z=z, cov=cov)
 
 
+def make_pose_graph_large(seed: int, n_nodes: int, n_edges: int, lattice: int, sigma_xy: float = 0.05,
+                          sigma_th: float = 0.02, min_gap: int = 50) -> dict:
+    """make_pose_graph's kind of graph at sizes its per-edge loops make slow (10^6 nodes): vectorised, with its own random
+    stream, so it does not reproduce make_pose_graph's graphs.  The lattice walk (1 m steps, 90 deg turns with probability
+    1/4 each way) is folded back into [0, lattice)^2 (a step across a border stays on its site) instead of turning; loop edges join nodes on the same or an
+    adjacent site with index gap > min_gap, drawn in rounds of one candidate per node until n_edges - (n_nodes - 1) distinct
+    pairs are found.  Measurements, covariances and the dead-reckoned initial guess as in make_pose_graph."""
+    rng = np.random.default_rng(seed)
+    r = rng.random(n_nodes - 1)
+    turn = np.where(r < 0.25, 1, np.where(r < 0.5, 3, 0))
+    head = np.concatenate([[0], np.cumsum(turn) % 4])
+    dirs = np.array([[1, 0], [0, 1], [-1, 0], [0, -1]])
+    raw = lattice // 2 + np.concatenate([np.zeros((1, 2), dtype=np.int64), np.cumsum(dirs[head[1:]], axis=0)])
+    period = 2 * lattice   # fold the unbounded walk into [0, lattice): a reflection at each border
+    m = np.mod(raw, period)
+    cell = np.where(m < lattice, m, period - 1 - m)
+    truth = np.column_stack([cell[:, 0].astype(float), cell[:, 1].astype(float), wrap(head * (math.pi / 2))])
+    key = cell[:, 0] * lattice + cell[:, 1]
+    order = np.argsort(key, kind="stable")
+    skey = key[order]
+    want = n_edges - (n_nodes - 1)
+    nb = np.array([(0, 0), (1, 0), (0, 1), (-1, 0), (0, -1)])
+    found = np.zeros(0, dtype=np.int64)
+    for _ in range(64):
+        if len(found) >= want:
+            break
+        i = rng.permutation(n_nodes)
+        c = cell[i] + nb[rng.integers(len(nb), size=n_nodes)]
+        ok = (c[:, 0] >= 0) & (c[:, 0] < lattice) & (c[:, 1] >= 0) & (c[:, 1] < lattice)
+        k = c[:, 0] * lattice + c[:, 1]
+        lo, hi = np.searchsorted(skey, k, "left"), np.searchsorted(skey, k, "right")
+        ok &= hi > lo
+        pick = lo + np.floor(rng.random(n_nodes) * np.maximum(hi - lo, 1)).astype(np.int64)
+        j = order[np.minimum(pick, n_nodes - 1)]
+        a, b = np.minimum(i, j), np.maximum(i, j)
+        ok &= (b - a) > min_gap
+        cand = np.concatenate([found, (a * n_nodes + b)[ok]])
+        _, first = np.unique(cand, return_index=True)
+        found = cand[np.sort(first)]
+    pairs = np.sort(found[:want])
+    ea = np.concatenate([np.arange(n_nodes - 1), pairs // n_nodes]).astype(np.int32)
+    eb = np.concatenate([np.arange(1, n_nodes), pairs % n_nodes]).astype(np.int32)
+    z = _pose_rel(truth[ea], truth[eb])
+    z += np.column_stack([rng.normal(0, sigma_xy, (len(ea), 2)), rng.normal(0, sigma_th, len(ea))])
+    z[:, 2] = wrap(z[:, 2])
+    t = -truth[ea, 2]
+    R = np.zeros((len(ea), 3, 3))
+    R[:, 0, 0] = np.cos(t); R[:, 0, 1] = -np.sin(t); R[:, 1, 0] = np.sin(t); R[:, 1, 1] = np.cos(t); R[:, 2, 2] = 1.0
+    cov = R @ np.diag([sigma_xy ** 2, sigma_xy ** 2, sigma_th ** 2]) @ R.transpose(0, 2, 1)
+    odo = z[: n_nodes - 1]
+    th = np.concatenate([[truth[0, 2]], truth[0, 2] + np.cumsum(odo[:, 2])])
+    c, s = np.cos(th[:-1]), np.sin(th[:-1])
+    init = np.zeros_like(truth)
+    init[0] = truth[0]
+    init[1:, 0] = truth[0, 0] + np.cumsum(c * odo[:, 0] - s * odo[:, 1])
+    init[1:, 1] = truth[0, 1] + np.cumsum(s * odo[:, 0] + c * odo[:, 1])
+    init[:, 2] = wrap(th)
+    return dict(ids=np.arange(n_nodes, dtype=np.int32), init=init, truth=truth, edge_a=ea, edge_b=eb, z=z, cov=cov)
+
+
 def _pose_rel(pa, pb):
     """pb in the frame of pa, rows (x, y, theta) -> (dx, dy, wrap(dtheta))."""
     c, s = np.cos(pa[:, 2]), np.sin(pa[:, 2])
