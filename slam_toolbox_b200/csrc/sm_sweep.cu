@@ -1356,7 +1356,14 @@ static int sweep_fetch(b200sm * h, bool do_refine, double * response, double * m
     int rc = build_plan(fg[p], h->probs_side, h->p, q, c2, foff, fres, 0.5 * h->p.coarse_angle_resolution,
                         h->p.fine_search_angle_offset, true, fp[p]);
     if (rc != B200_OK) return rc;
-    P = fp[p].nX * fp[p].nY; nA = fp[p].nA;
+    // every pair's offsets, positions and sums are laid out with pair 0's plan size (the window and the angles are the same for
+    // every pair, only the centre differs): a plan of another size would misplace its own and its neighbours' entries
+    if (p == 0) {
+      P = fp[0].nX * fp[0].nY; nA = fp[0].nA;
+    } else if (fp[p].nX != fp[0].nX || fp[p].nY != fp[0].nY || fp[p].nA != nA) {
+      set_last_error("sweep: fine plans of one batch differ in size");
+      return B200_ERR_UNSUPPORTED;
+    }
   }
   const int n = S.n;
   const size_t no = (size_t)S.npairs * nA * n, np = (size_t)S.npairs * P, ns = (size_t)S.npairs * P * nA;
