@@ -45,6 +45,10 @@ constexpr int kRowTiles = 6;           // register pairs of 16-bit fields per th
 constexpr int kChunkBeams = 640;       // beams accumulated in 16-bit fields before a flush (640 * 100 < 65536)
 constexpr int kMaxSingles = 63;        // weighted singles of one item (6-bit field of the item record, sm_types.cuh)
 constexpr int kMaxPairs = 255;         // weighted pairs of one item (8-bit field)
+// guard words before / after the accumulator volume A: the flush adds zero to columns -3 .. 16 * xtiles - 1 <= nX + 17 of a row, so
+// the first row reaches 3 words before A and the last row 18 words past it
+constexpr int kAGuardLo = 4;
+constexpr int kAGuardHi = 20;
 
 // ------------------------------------------------------------------------------------------
 // PTX helpers: mbarrier, bulk async copy (TMA 1-D), cluster barrier, distributed shared memory
@@ -110,6 +114,13 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t a)
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a));
   return v;
+}
+
+// shared-memory reduction without a result.  The flush issues it unconditionally: ptxas wraps every lane-dependent shared atomic,
+// predicated PTX included, in a BSSY / BRA / BSYNC region of its own
+__device__ __forceinline__ void red_add(uint32_t a, uint32_t v)
+{
+  asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
 }
 
 __device__ __forceinline__ uint32_t even_bytes_t(uint32_t w) { return __byte_perm(w, 0, 0x4240); }   // [b0, 0, b2, 0]
@@ -378,12 +389,16 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
         // are dropped at the flush (y >= y_end) -- so a band needs a halo of nY rows, not of whole y-tiles, and the row offsets
         // stay warp-uniform (LDS [R + UR]).
         const int x0 = 4 * (4 * xt + j_l) - m;
-        auto add4 = [&](int32_t * dst, uint32_t t0, uint32_t t1) {
-          const int v0 = t0 & 0xFFFF, v1 = t1 & 0xFFFF, v2 = t0 >> 16, v3 = t1 >> 16;
-          if (v0 && (unsigned)(x0 + 0) < (unsigned)nX) atomicAdd(dst + 0, v0);
-          if (v1 && (unsigned)(x0 + 1) < (unsigned)nX) atomicAdd(dst + 1, v1);
-          if (v2 && (unsigned)(x0 + 2) < (unsigned)nX) atomicAdd(dst + 2, v2);
-          if (v3 && (unsigned)(x0 + 3) < (unsigned)nX) atomicAdd(dst + 3, v3);
+        // The flush is straight-line code: every lane reduces all of its fields, and a field that is not a pose of this item adds
+        // zero.  The lane's four x-range tests are fixed for the item and become masks of the two packed words (T0 holds the
+        // fields of x0 and x0 + 2, T1 those of x0 + 1 and x0 + 3); a row beyond the last pose row is masked to zero and its
+        // address clamped to the last one.  Columns -3 .. nX + 17 of a row stay inside the angle's volume or the guard words
+        // around A (kAGuardLo / kAGuardHi), so every address is one the item may add zero to.
+        auto add4 = [&](uint32_t a, uint32_t t0, uint32_t t1) {
+          red_add(a + 0, t0 & 0xFFFFu);
+          red_add(a + 4, t1 & 0xFFFFu);
+          red_add(a + 8, t0 >> 16);
+          red_add(a + 12, t1 >> 16);
         };
         auto flush = [&](const uint32_t (&T0)[kRowTiles], const uint32_t (&T1)[kRowTiles]) {
           TILE_TM(kTmCorr);
@@ -391,22 +406,34 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
 #pragma unroll
           for (int r = 0; r < kRowTiles; ++r) any |= T0[r] | T1[r];
           if (!__any_sync(0xffffffffu, any != 0)) { TILE_TM(kTmFlush); return; }
-#pragma unroll
-          for (int r = 0; r < kMain; ++r) {
-            const int y = ybase + 8 * r;
-            if (y >= y_end || (T0[r] | T1[r]) == 0) continue;
-            add4(Arow + y * nX + x0, T0[r], T1[r]);
-          }
-          if (tail) {
-            // the tail row's fields of the 8 lane-rows of a word column: three butterfly adds (the item's whole weight fits
-            // 16 bits), lane-row 0 adds them
-            uint32_t t0 = T0[kRowTiles - 1], t1 = T1[kRowTiles - 1];
+          // the tail row's fields of the 8 lane-rows of a word column: three butterfly adds (the item's whole weight fits 16 bits)
+          // ahead of the first reduction, so that no convergence check splits the reductions.  Zero outside the last y-tile, so
+          // every item of the tail layout runs it unbranched.
+          uint32_t t0 = 0, t1 = 0;
+          if (kTail) {
+            t0 = T0[kRowTiles - 1]; t1 = T1[kRowTiles - 1];
 #pragma unroll
             for (int o = 4; o < 32; o <<= 1) {
               t0 += __shfl_xor_sync(0xffffffffu, t0, o);
               t1 += __shfl_xor_sync(0xffffffffu, t1, o);
             }
-            if (y_l == 0 && (t0 | t1) != 0) add4(Arow + (nY - 1) * nX + x0, t0, t1);
+          }
+          const uint32_t xm0 = ((unsigned)x0 < (unsigned)nX ? 0x0000FFFFu : 0u) | ((unsigned)(x0 + 2) < (unsigned)nX ? 0xFFFF0000u : 0u);
+          const uint32_t xm1 = ((unsigned)(x0 + 1) < (unsigned)nX ? 0x0000FFFFu : 0u) | ((unsigned)(x0 + 3) < (unsigned)nX ? 0xFFFF0000u : 0u);
+          const uint32_t ax = smem_u32(Arow) + 4u * (uint32_t)x0, rowB = 4u * (uint32_t)nX;   // x0 >= -3: modular, into the guard
+          const int ylast = max(y_end - 1, 0);
+#pragma unroll
+          for (int r = 0; r < kMain; ++r) {
+            const int y = ybase + 8 * r;
+            const uint32_t rm = y < y_end ? ~0u : 0u;
+            add4(ax + rowB * (uint32_t)min(y, ylast), T0[r] & xm0 & rm, T1[r] & xm1 & rm);
+          }
+          if (kTail) {
+            // lane-row 0 (ybase == kYTile * yt) adds the tail row, the other lane-rows add zero to rows of their own (no
+            // same-address atomics)
+            const bool tv = tail && ybase == kYTile * yt;
+            const uint32_t tm = tv ? ~0u : 0u;
+            add4(ax + rowB * (uint32_t)(tv ? nY - 1 : min(ybase, ylast)), t0 & xm0 & tm, t1 & xm1 & tm);
           }
           TILE_TM(kTmFlush);
         };
@@ -957,7 +984,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     if (force_v > 0 && V < std::min(force_v, nA)) continue;   // "sweep_chunks" = at least this many chunks
     const int nAc = (nA + V - 1) / V;
     if ((nA + nAc - 1) / nAc != V || nAc > 63) continue;   // same chunk size as a smaller V; group ids are bytes
-    const int a_bytes = (nAc * P * 4 + 15) & ~15;
+    const int a_bytes = (4 * (kAGuardLo + nAc * P + kAGuardHi) + 15) & ~15;
     // staging buffer: item list + 1.5 x the average descriptor bytes of a (chunk, phase) block, at least one angle's worst case:
     // one item record per (alignment, tile), plus one per tile for every further kChunkBeams-piece of a long group -- the
     // groups of one angle hold at most n beams, so they are cut at most (n - 1) / kChunkBeams more times
@@ -977,11 +1004,13 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     const int nbv = (base_rows + B - 1) / B;
     B = (base_rows + nbv - 1) / nbv;                     // even bands
     // cost of one pair on one CTA, in thread-instructions: rasters (4 phases per chunk and band) + the beam loop per angle
-    // the accumulator flush of every (angle, stage, alignment, tile) item (~100 warp instructions each, 32 warps) and the fixed
-    // cost of a stage (clear + raster + three barriers) are what make extra bands expensive
+    // the accumulator flush of every (angle, stage, alignment, tile) item (32 warps) and the fixed cost of a stage (clear + raster +
+    // three barriers) are what make extra bands expensive.  The flush is straight-line code: 124 warp instructions from the vote to
+    // the last reduction on the tail layout, 112 on 48-row y-tiles (sm_90a SASS of k_sweep_tile)
     // the beam loop: ~2.3 thread-instructions per lane and row-tile load (6 per beam and 48-row y-tile; 5 + 2 / 8 with the tail)
     const double loads = tail ? 5.0 * ytiles + 0.25 : 6.0 * ytiles;
-    const long w_angle = (long)((double)n * xtiles * loads * 32 * 2.3 / kTileThreads) + 4L * nbv * (4L * xtiles * ytiles * 100 / 32);
+    const long flush_wi = tail ? 124 : 112;
+    const long w_angle = (long)((double)n * xtiles * loads * 32 * 2.3 / kTileThreads) + 4L * nbv * (4L * xtiles * ytiles * flush_wi / 32);
     const long w_raster = 4 * (700 + 3L * std::min(B + halo, rows_valid + halo - nY) * pitch_w / kTileThreads);
     const long cost = (long)((V + Cc - 1) / Cc) * (nbv * w_raster + nAc * w_angle);
     if (bestCost < 0 || cost < bestCost) { bestCost = cost; bestV = V; bestNb = nbv; bestB = B; bestStage = stage; }
@@ -992,7 +1021,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   int alloc_rows = std::min(B + halo, rows_valid + halo - nY);
   alloc_rows = std::max(alloc_rows, 1);
   const size_t s_bytes = ((size_t)alloc_rows * pitch_w * 4 + 15) & ~(size_t)15;
-  const size_t a_bytes = ((size_t)nAc * P * 4 + 15) & ~(size_t)15;
+  const size_t a_bytes = (4 * ((size_t)kAGuardLo + (size_t)nAc * P + kAGuardHi) + 15) & ~(size_t)15;   // A and its guard words
   T.C = C; T.V = V; T.nAc = nAc; T.nbands = nbands; T.band_rows = B; T.alloc_rows = alloc_rows; T.pitch_w = pitch_w;
   T.xtiles = xtiles; T.ytiles = ytiles; T.tail = tail ? 1 : 0; T.stage_bytes = stage_bytes;
   T.int_ties = int_ties;
@@ -1005,7 +1034,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     T.nlevels = (!lv.empty() && lv.size() <= 4) ? (int)lv.size() : 0;
     for (int i = 0; i < 4; ++i) T.level[i] = i < T.nlevels ? lv[i] : 0;
   }
-  T.off_A = s_bytes; T.off_probs = s_bytes + a_bytes; T.off_stage = (T.off_probs + probs_bytes + 127) & ~(size_t)127;
+  T.off_A = s_bytes + 4 * kAGuardLo; T.off_probs = s_bytes + a_bytes; T.off_stage = (T.off_probs + probs_bytes + 127) & ~(size_t)127;
   T.off_cells = T.off_stage + 2 * (size_t)stage_bytes;
   // cell-list staging only where the chosen plan leaves room for it (it must not cost a band or a chunk)
   int cell_cap = d_max_n_ok(S.max_n) ? S.max_n : 0;                     // entries per cell staging buffer (0 = read cells from global)

@@ -4,7 +4,7 @@ Builds the library with -DB200_TILE_TIMERS into a scratch directory (the shipped
 bench's cfg2 loop-closure batch (1 query x N candidates, +-2 m / +-20 deg, 41 x 41 x 21 poses) or another geometry,
 and prints every section as a share of the warp cycles of the launch and as SM cycles per pair.
 
-usage: tile_timers.py [--n 1000] [--geom 4:12] [--runs 5] [--build-dir DIR] [--json OUT]
+usage: tile_timers.py [--n 1000] [--geom 4:12] [--runs 5] [--build-dir DIR [--reuse]] [--json OUT]
 """
 import argparse
 import ctypes as C
@@ -47,12 +47,14 @@ def main():
     ap.add_argument("--geom", default="4:12", help="search dimension [m]:range threshold [m]")
     ap.add_argument("--runs", type=int, default=5, help="timed launches (after one warm-up)")
     ap.add_argument("--build-dir", default=None, help="where the instrumented library goes (default: a temporary directory)")
+    ap.add_argument("--reuse", action="store_true", help="take the instrumented library already in --build-dir")
     ap.add_argument("--json", default=None, help="also write the result here")
     a = ap.parse_args()
 
     build_dir = a.build_dir or tempfile.mkdtemp(prefix="b200_tile_timers_")
     os.makedirs(build_dir, exist_ok=True)
-    _build.LIB = build_instrumented(build_dir)
+    prebuilt = os.path.join(build_dir, "libb200slam_timers.so")
+    _build.LIB = prebuilt if (a.reuse and os.path.exists(prebuilt)) else build_instrumented(build_dir)
     import bench
     from slam_toolbox_b200 import api
     L = api.lib()
