@@ -89,6 +89,7 @@ public:
     b200pg_summary s;
     if (b200pg_solve(h_, &s) != B200_OK) return;   // unusable: corrections untouched, like the reference
     solve_ms_ += s.solve_ms;
+    compute_log_.push_back({s.solve_ms, s.uploaded_edges});
     const int n = b200pg_num_nodes(h_);
     std::vector<int32_t> ids(n);
     std::vector<double> p(3 * (size_t)n);
@@ -161,6 +162,11 @@ public:
 
   int computes() const { return computes_; }
   double solve_ms() const { return solve_ms_; }
+  // one record per successful Compute: device ms of the solve and the constraints it uploaded (all of them after a removal)
+  struct ComputeRecord { double solve_ms; int uploaded_edges; };
+  const std::vector<ComputeRecord> & compute_log() const { return compute_log_; }
+  int num_nodes() const { std::lock_guard<std::mutex> lock(mu_); return b200pg_num_nodes(h_); }
+  int num_edges() const { std::lock_guard<std::mutex> lock(mu_); return b200pg_num_edges(h_); }
 
 private:
   mutable std::mutex mu_;                                 // mirrors CeresSolver::nodes_mutex_
@@ -170,6 +176,7 @@ private:
   std::unordered_map<int, Eigen::Vector3d> graph_;
   int computes_ = 0;
   double solve_ms_ = 0.0;
+  std::vector<ComputeRecord> compute_log_;
 };
 
 }  // namespace solver_plugins

@@ -2,6 +2,9 @@
 // scans, with the GPU ScanSolver adapter installed through Mapper::SetScanSolver and -- when linked into
 // libreplay_b200.so -- every MatchScan redirected to the GPU by scan_matcher_b200.cpp.
 // libreplay_ref.so is the same driver linked WITHOUT the matcher shim (reference CPU matcher).
+// Localization mode (src/slam_toolbox_localization.cpp:176-237) runs through the same mapper: ProcessLocalization,
+// ProcessAgainstNodesNearBy and ClearLocalizationBuffer.  There the mapper deletes the scans it drops from its rolling
+// buffer, so the driver holds no scan pointers of its own: every readout walks the mapper's current processed set.
 #include <chrono>
 #include <csignal>
 #include <cstdlib>
@@ -19,11 +22,52 @@ namespace {
 struct Replay {
   Mapper mapper;
   solver_plugins::B200Solver * solver = nullptr;
-  std::vector<LocalizedRangeScan *> scans;
   double process_seconds = 0.0;
-  int processed = 0;
 };
 const char * kLaser = "laser0";
+
+// a new scan at the odometric pose, corrected pose = odometric pose (SlamToolbox::getLocalizedRangeScan)
+LocalizedRangeScan * make_scan(const double * ranges, int n, const double odom[3], int id)
+{
+  RangeReadingsVector rr(ranges, ranges + n);
+  LocalizedRangeScan * s = new LocalizedRangeScan(Name(kLaser), rr);
+  Pose2 p(odom[0], odom[1], odom[2]);
+  s->SetOdometricPose(p);
+  s->SetCorrectedPose(p);
+  s->SetTime(static_cast<double>(id));
+  return s;
+}
+
+// the scans the mapper holds now (Mapper::GetAllProcessedScans: unique-id order, which is processing order)
+LocalizedRangeScanVector processed_scans(Replay * r) { return r->mapper.GetAllProcessedScans(); }
+
+// The localization calls remove nodes through m_pScanOptimizer without a check (Mapper.cpp:2977, 3003), and a rolling
+// buffer of 0 scans would delete the scan being processed before the caller reads its pose.
+bool can_localize(Replay * r) { return r->solver != nullptr && r->mapper.getParamScanBufferSize() >= 1; }
+
+// runs one mapper call on a new scan; the scan is the mapper's once processed, else deleted.  Writes the corrected pose and
+// the covariance the localization node publishes (slam_toolbox_localization.cpp:195-233).
+template <class F>
+int run_scan(Replay * r, LocalizedRangeScan * s, const char * what, F && call, double * out_pose, double * out_cov)
+{
+  Matrix3 cov;
+  cov.SetToIdentity();
+  auto t0 = std::chrono::steady_clock::now();
+  bool ok = false;
+  try {
+    ok = call(s, &cov);
+  } catch (const std::exception & e) {
+    std::fprintf(stderr, "%s: %s\n", what, e.what());
+  }
+  r->process_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  if (!ok) { delete s; return 0; }
+  if (out_pose) {
+    const Pose2 & p = s->GetCorrectedPose();
+    out_pose[0] = p.GetX(); out_pose[1] = p.GetY(); out_pose[2] = p.GetHeading();
+  }
+  if (out_cov) for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) out_cov[3 * i + j] = cov(i, j);
+  return 1;
+}
 }
 
 static void segv_handler(int)
@@ -120,6 +164,13 @@ int krep_set(void * rp, const char * name, double v)
   else if (n == "use_scan_barycenter") m->setParamUseScanBarycenter(v != 0.0);
   else if (n == "minimum_time_interval") m->setParamMinimumTimeInterval(v);
   else return -1;
+  // After the first scan the running-scan buffer has its own copy of the two buffer limits.  Hand it the new ones as
+  // Mapper::Initialize does for a loaded map (Mapper.cpp:2620-2623), the way the localization node starts on a map:
+  // a localization buffer shorter than the running buffer would otherwise leave deleted scans among the running scans.
+  if (MapperSensorManager * sm = m->GetMapperSensorManager()) {
+    if (n == "scan_buffer_size") sm->SetRunningScanBufferSize(static_cast<kt_int32u>(v));
+    else if (n == "scan_buffer_maximum_scan_distance") sm->SetRunningScanBufferMaximumDistance(v);
+  }
   return 0;
 }
 
@@ -127,34 +178,109 @@ int krep_set(void * rp, const char * name, double v)
 int krep_process(void * rp, const double * ranges, int n, const double odom[3], int id)
 {
   Replay * r = static_cast<Replay *>(rp);
-  RangeReadingsVector rr(ranges, ranges + n);
-  LocalizedRangeScan * s = new LocalizedRangeScan(Name(kLaser), rr);
-  Pose2 p(odom[0], odom[1], odom[2]);
-  s->SetOdometricPose(p);
-  s->SetCorrectedPose(p);
-  s->SetTime(static_cast<double>(id));
-  auto t0 = std::chrono::steady_clock::now();
-  bool ok = false;
-  try {
-    ok = r->mapper.Process(s);
-  } catch (const std::exception & e) {
-    std::fprintf(stderr, "krep_process: %s\n", e.what());
-  }
-  r->process_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-  if (ok) { r->scans.push_back(s); ++r->processed; } else { delete s; }
-  return ok ? 1 : 0;
+  return run_scan(r, make_scan(ranges, n, odom, id), "krep_process",
+                  [r](LocalizedRangeScan * s, Matrix3 *) { return r->mapper.Process(s); }, nullptr, nullptr);
 }
 
-int krep_num_scans(void * rp) { return static_cast<int>(static_cast<Replay *>(rp)->scans.size()); }
-
-// corrected poses (after all loop closures) of the processed scans, in processing order
-void krep_poses(void * rp, double * out)
+// Mapper::ProcessLocalization (Mapper.cpp:2831-2909), the localization node's PROCESS_LOCALIZATION step.  Returns 1 if the
+// scan was processed (out_pose = its corrected pose, out_cov = the published covariance), 0 if not, -1 (nothing done)
+// without a solver or with scan_buffer_size < 1.
+int krep_process_localization(void * rp, const double * ranges, int n, const double odom[3], int id, double out_pose[3],
+                              double out_cov[9])
 {
   Replay * r = static_cast<Replay *>(rp);
-  for (size_t i = 0; i < r->scans.size(); ++i) {
-    const Pose2 & p = r->scans[i]->GetCorrectedPose();
+  if (!can_localize(r)) return -1;
+  return run_scan(r, make_scan(ranges, n, odom, id), "krep_process_localization",
+                  [r](LocalizedRangeScan * s, Matrix3 * c) { return r->mapper.ProcessLocalization(s, c); }, out_pose, out_cov);
+}
+
+// PROCESS_NEAR_REGION (slam_toolbox_localization.cpp:197-212): the scan's odometric and corrected pose are set to the
+// requested pose, then Mapper::ProcessAgainstNodesNearBy(scan, true, &cov) matches it against the map scan nearest to it
+// and puts it in the rolling buffer.  Returns as krep_process_localization.
+int krep_process_near(void * rp, const double * ranges, int n, const double odom[3], int id, const double pose[3],
+                      double out_pose[3], double out_cov[9])
+{
+  Replay * r = static_cast<Replay *>(rp);
+  if (!can_localize(r)) return -1;
+  LocalizedRangeScan * s = make_scan(ranges, n, odom, id);
+  const Pose2 p(pose[0], pose[1], pose[2]);
+  s->SetOdometricPose(p);
+  s->SetCorrectedPose(p);
+  return run_scan(r, s, "krep_process_near",
+                  [r](LocalizedRangeScan * s, Matrix3 * c) { return r->mapper.ProcessAgainstNodesNearBy(s, true, c); },
+                  out_pose, out_cov);
+}
+
+// Mapper::ClearLocalizationBuffer (Mapper.cpp:2937-2962): every buffered scan leaves the graph and the solver, and the
+// running and last scans are cleared.  0 on success, -1 (nothing done) without a solver or before the first scan.
+int krep_clear_localization_buffer(void * rp)
+{
+  Replay * r = static_cast<Replay *>(rp);
+  if (!can_localize(r) || !r->mapper.GetMapperSensorManager()) return -1;
+  r->mapper.ClearLocalizationBuffer();
+  return 0;
+}
+
+int krep_num_scans(void * rp) { return static_cast<int>(processed_scans(static_cast<Replay *>(rp)).size()); }
+
+// corrected poses (after all loop closures) of the scans the mapper holds, in processing order; ids (if not NULL) receives
+// their unique ids.  krep_num_scans gives the count.
+void krep_poses(void * rp, double * out, int * ids)
+{
+  const LocalizedRangeScanVector v = processed_scans(static_cast<Replay *>(rp));
+  for (size_t i = 0; i < v.size(); ++i) {
+    const Pose2 & p = v[i]->GetCorrectedPose();
     out[3 * i] = p.GetX(); out[3 * i + 1] = p.GetY(); out[3 * i + 2] = p.GetHeading();
+    if (ids) ids[i] = v[i]->GetUniqueId();
   }
+}
+
+// the mapper's graph edges (MapperGraph::GetEdges, insertion order): source / target unique ids, LinkInfo pose difference
+// and covariance (row-major), filled up to cap.  Returns the number of edges.
+int krep_edges(void * rp, int * src, int * dst, double * diff, double * cov, int cap)
+{
+  Replay * r = static_cast<Replay *>(rp);
+  if (!r->mapper.GetGraph()) return 0;
+  const std::vector<Edge<LocalizedRangeScan> *> & edges = r->mapper.GetGraph()->GetEdges();
+  int k = 0;
+  for (Edge<LocalizedRangeScan> * e : edges) {
+    if (k < cap) {
+      LinkInfo * li = static_cast<LinkInfo *>(e->GetLabel());
+      src[k] = e->GetSource()->GetObject()->GetUniqueId();
+      dst[k] = e->GetTarget()->GetObject()->GetUniqueId();
+      const Pose2 d = li->GetPoseDifference();
+      const Matrix3 c = li->GetCovariance();
+      diff[3 * k] = d.GetX(); diff[3 * k + 1] = d.GetY(); diff[3 * k + 2] = d.GetHeading();
+      for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) cov[9 * k + 3 * i + j] = c(i, j);
+    }
+    ++k;
+  }
+  return k;
+}
+
+// graph sizes: mapper vertices, mapper edges, solver nodes, solver edges (the solver's are -1 without one)
+void krep_counts(void * rp, int out[4])
+{
+  Replay * r = static_cast<Replay *>(rp);
+  MapperGraph * g = r->mapper.GetGraph();
+  int nv = 0;
+  if (g)
+    for (const auto & kv : g->GetVertices()) nv += static_cast<int>(kv.second.size());
+  out[0] = nv;
+  out[1] = g ? static_cast<int>(g->GetEdges().size()) : 0;
+  out[2] = r->solver ? r->solver->num_nodes() : -1;
+  out[3] = r->solver ? r->solver->num_edges() : -1;
+}
+
+// per Compute of the adapter, in call order: device ms of the solve and the constraints it uploaded; filled up to cap.
+// Returns the number of computes.
+int krep_solver_computes(void * rp, double * ms, int * uploaded, int cap)
+{
+  Replay * r = static_cast<Replay *>(rp);
+  if (!r->solver) return 0;
+  const auto & log = r->solver->compute_log();
+  for (size_t i = 0; i < log.size() && static_cast<int>(i) < cap; ++i) { ms[i] = log[i].solve_ms; uploaded[i] = log[i].uploaded_edges; }
+  return static_cast<int>(log.size());
 }
 
 // ScanSolver::getGraph() of the adapter: number of nodes; ids / poses filled up to cap
@@ -179,7 +305,7 @@ void krep_stats(void * rp, double out[5])
   out[1] = r->solver ? r->solver->computes() : 0;
   out[2] = r->solver ? r->solver->solve_ms() : 0;
   out[3] = static_cast<double>(r->mapper.GetGraph() ? r->mapper.GetGraph()->GetEdges().size() : 0);
-  out[4] = static_cast<double>(r->scans.size());
+  out[4] = static_cast<double>(processed_scans(r).size());
 }
 
 // map publish over all processed scans (SMapper::getOccupancyGrid, src/slam_mapper.cpp:63-69):
@@ -188,7 +314,7 @@ void krep_stats(void * rp, double out[5])
 double krep_occupancy(void * rp, double resolution, int use_gpu, int info[3], double offset[2], unsigned char * cells, long cap)
 {
   Replay * r = static_cast<Replay *>(rp);
-  LocalizedRangeScanVector v(r->scans.begin(), r->scans.end());
+  const LocalizedRangeScanVector v = processed_scans(r);
   auto t0 = std::chrono::steady_clock::now();
   OccupancyGrid * g = use_gpu ? karto::b200::CreateOccupancyGridFromScans(v, resolution) : OccupancyGrid::CreateFromScans(v, resolution);
   const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
