@@ -23,6 +23,8 @@ UNITS = {
     "sm_sweep.cu": ["-fmad=false"],
     "sm_tile.cu": ["-fmad=false"],
     "pose_graph.cu": [],
+    "pg_pcg.cu": [],
+    "pg_cholesky.cu": [],
     "occupancy.cu": ["-fmad=false"],
 }
 

@@ -7,7 +7,9 @@
 #include <cstddef>
 #include <cstdint>
 #include <cstdio>
+#include <exception>
 #include <functional>
+#include <new>
 #include <string>
 
 #include "../../include/b200slam.h"
@@ -29,6 +31,15 @@ struct CudaFail {
       throw ::b200::CudaFail{B200_ERR_CUDA};                                                  \
     }                                                                                         \
   } while (0)
+
+// Around the body of a C ABI entry: a failed CUDA call, an exhausted host heap or any other exception becomes its error
+// code (and the last error message) instead of crossing the C boundary.
+#define B200_GUARD_BEGIN try {
+#define B200_GUARD_END                                                     \
+  }                                                                        \
+  catch (const b200::CudaFail & f) { return f.code; }                      \
+  catch (const std::bad_alloc &) { b200::set_last_error("out of host memory"); return B200_ERR_CUDA; } \
+  catch (const std::exception & e) { b200::set_last_error(e.what()); return B200_ERR_CUDA; }
 
 // Fails loudly (B200_ERR_CUDA) when there is no sm_90 device: there is no CPU fallback.
 void require_device();

@@ -492,13 +492,6 @@ int build(b200og * h, b200og_info * info)
 
 }  // namespace
 
-#define B200_GUARD_BEGIN try {
-#define B200_GUARD_END                                                     \
-  }                                                                        \
-  catch (const b200::CudaFail & f) { return f.code; }                      \
-  catch (const std::bad_alloc &) { b200::set_last_error("out of host memory"); return B200_ERR_CUDA; } \
-  catch (const std::exception & e) { b200::set_last_error(e.what()); return B200_ERR_CUDA; }
-
 extern "C" {
 
 void b200og_default_params(b200og_params * p)

@@ -821,13 +821,6 @@ double do_match(b200sm * h, const b200_scan * query, const b200_scan * base, int
 // ------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------
-#define B200_GUARD_BEGIN try {
-#define B200_GUARD_END                                                     \
-  }                                                                        \
-  catch (const b200::CudaFail & f) { return f.code; }                      \
-  catch (const std::bad_alloc &) { b200::set_last_error("out of host memory"); return B200_ERR_CUDA; } \
-  catch (const std::exception & e) { b200::set_last_error(e.what()); return B200_ERR_CUDA; }
-
 extern "C" {
 
 const char * b200_last_error(void) { return g_last_error.c_str(); }

@@ -1405,13 +1405,6 @@ static int sweep_fetch(b200sm * h, bool do_refine, double * response, double * m
 
 using namespace b200;
 
-#define B200_GUARD_BEGIN try {
-#define B200_GUARD_END                                                     \
-  }                                                                        \
-  catch (const b200::CudaFail & f) { return f.code; }                      \
-  catch (const std::bad_alloc &) { b200::set_last_error("out of host memory"); return B200_ERR_CUDA; } \
-  catch (const std::exception & e) { b200::set_last_error(e.what()); return B200_ERR_CUDA; }
-
 extern "C" {
 
 int b200sm_batch_upload(b200sm * h, const b200_scan * queries, int32_t nq, const b200_scan * scans, int32_t nscans,

@@ -1,4 +1,4 @@
-"""Plain FP64 restatement of the pose-graph solver's PCG linear solve (pose_graph.cu: k_pg_pcg, k_pg_pcg_smem, k_pg_pcg_2lvl and
+"""Plain FP64 restatement of the pose-graph solver's PCG linear solve (pg_pcg.cu: k_pg_pcg, k_pg_pcg_smem, k_pg_pcg_2lvl and
 k_pg_pcg_2lvl_g), written from the kernels, for tests that compare the solver iterate by iterate.
 
 The system is the LM step's Jacobi-scaled normal equations over all N nodes in insertion order,

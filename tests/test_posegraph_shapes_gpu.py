@@ -62,7 +62,7 @@ def degrees(n, ia, ib):
 
 
 def planned_kernel(deg, sms, coarse_modes=6, precond=1, force_global=False):
-    """The host plan of pose_graph.cu (plan_pcg(): shared-memory Jacobi bytes, then the two-level aggregates and their
+    """The host plan of pg_pcg.cu (plan_pcg(): shared-memory Jacobi bytes, then the two-level aggregates and their
     bytes for 6 and 3 coarse modes) restated from the node degrees in insertion order."""
     N = len(deg)
     start = np.concatenate([[0], np.cumsum(deg)])

@@ -51,7 +51,7 @@ def main():
     objs = []
     for unit, extra in B.UNITS.items():
         obj = os.path.join(tmp, unit.replace(".cu", ".o"))
-        flags = extra + (["-DB200_CHOL_CHECKS"] if unit == "pose_graph.cu" else [])
+        flags = extra + (["-DB200_CHOL_CHECKS"] if unit == "pg_cholesky.cu" else [])
         subprocess.run(["nvcc"] + B.ARCH + B.COMMON + flags + ["-c", os.path.join(B.CSRC, unit), "-o", obj], check=True)
         objs.append(obj)
     lib = os.path.join(tmp, "libb200slam.so")

@@ -8,7 +8,7 @@ nodes; and 1,000,000 nodes / 4,000,000 edges from the vectorised synth.make_pose
 5 iterations (both kernels run the same steps; a full solve of kernel 0 there takes minutes).  On each graph the default
 plan and forced kernel 0 run alternately on fresh handles (--reps of each).  Every row records the planned kernel, LM iterations,
 accepted steps, linear solves, total CG iterations, device ms and device ms per CG iteration (whole solve / CG
-iterations), for the global two-level kernel the aggregate size and coarse size nc (pose_graph.cu's rule restated in
+iterations), for the global two-level kernel the aggregate size and coarse size nc (pg_pcg.cu's rule restated in
 coarse_plan; tests/test_posegraph_large_gpu.py checks it against the plan the solver prints), and the algorithmic bytes of
 one CG iteration (fine level and the dense coarse mat-vec) over the time per iteration, against the data-sheet HBM3
 bandwidth (3.35 TB/s).  Working sets of a few tens of MB sit in L2, so that ratio is a bandwidth share only where the
@@ -51,7 +51,7 @@ GRAPHS = {
 
 
 def coarse_plan(n, e, cm=6):
-    """pose_graph.cu coarse_aggregates_2lvl_global(): nc <= sqrt(fine bytes / 32), at most 4096, aggregates >= 16 nodes."""
+    """pg_pcg.cu coarse_aggregates_2lvl_global(): nc <= sqrt(fine bytes / 32), at most 4096, aggregates >= 16 nodes."""
     fine = 240.0 * n + 128.0 * 2 * e
     nc = min(4096, int(math.sqrt(fine / 32.0)))
     want = max(1, min((n + 15) // 16, nc // cm))
