@@ -21,6 +21,7 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-ffp-contract=o
 UNITS = {
     "scan_matcher.cu": ["-fmad=false"],
     "sm_sweep.cu": ["-fmad=false"],
+    "sm_fast.cu": ["-fmad=false"],
     "sm_tile.cu": ["-fmad=false"],
     "pose_graph.cu": [],
     "pg_pcg.cu": [],

@@ -1,4 +1,4 @@
-// b200slam scan matcher, batched loop-closure sweep (generic path).
+// b200slam scan matcher, batched loop-closure sweep: the generic kernel, the host side and the batch C ABI.
 //
 // Reference: MapperGraph::TryCloseLoop (lib/karto_sdk/src/Mapper.cpp:1500-1561) calls
 // ScanMatcher::MatchScan once per candidate chain; here every (query, chain) pair of a sweep is
@@ -7,6 +7,9 @@
 //   k_sweep_generic  per pair: clear + smear raster, exhaustive correlation, arg-max / ties /
 //                    positional-covariance accumulators                          (M.cpp:641-966)
 //   k_sweep_fine     3x3xnA fine volumes for do_refine                           (M.cpp:621-629)
+//   k_best_keys, k_win_*  per-query keys / winner records of the multi-GPU sweep
+// The host side uploads a sweep, chooses its kernel once (the parity-sub-grid kernels live in sm_fast.cu and
+// sm_tile.cu), runs it and finishes the pairs.
 // Compile with -fmad=false / -ffp-contract=off (bit-exact FP64, see sm_math.cuh).
 #include <algorithm>
 #include <chrono>
@@ -23,7 +26,7 @@
 namespace b200 {
 
 // ------------------------------------------------------------------------------------------
-// batch sweep, generic path
+// batch sweep, generic kernel
 // ------------------------------------------------------------------------------------------
 
 // ScanMatcher::FindValidPoints (M.cpp:1113-1164) + WorldToGrid + ROI test (M.cpp:1082-1088) for
@@ -112,109 +115,34 @@ __global__ void __launch_bounds__(kFvWarps * 32) k_find_valid(SweepDev d)
   if (lane == 0) d.cell_count[item] = total;
 }
 
-// The on-device part of CorrelateScan's reduction (M.cpp:775-829) and of
-// ComputePositionalCovariance (M.cpp:893-933) for one pair whose integer volume is in `sums`
-// (index (y*nX+x)*nA + a).  `probs` = P doubles of scratch.  Everything that needs libm
-// (heading average) is finished on the host from the tie list.
-struct SumsPoseMajor {   // generic path: volume index (y*nX + x)*nA + a in global memory
-  const int32_t * v; int nA;
-  __device__ __forceinline__ int operator()(int p, int a) const { return v[(size_t)p * nA + a]; }
-};
-struct SumsAngleMajor {  // fast path: accumulators [a][y*nX + x] in shared memory
-  const int32_t * v; int P;
-  __device__ __forceinline__ int operator()(int p, int a) const { return v[a * P + p]; }
-};
-
-template <class SumAt>
-__device__ void pair_epilogue(const SweepDev & d, int pair, int q, const SumAt sums,
-                              double * probs, double * s_dscratch, int * s_iscratch)
+// Grid::Clear (M.cpp:1034) of a CTA's workspace grid
+__device__ __forceinline__ void clear_grid(const SweepDev & d, uint8_t * grid)
 {
-  const int P = d.nX * d.nY, nA = d.nA;
-  PairOut & out = d.out[pair];
-  // best response + per-cell max over angles (the m_pSearchSpaceProbs image, M.cpp:781-799)
-  double lbest = -1.0;
-  for (int p = threadIdx.x; p < P; p += blockDim.x) {
-    const int x = p % d.nX, y = p / d.nX;
-    double pm = 0.0;   // Grid<double>::Clear() initial value, M.cpp:727
-    for (int a = 0; a < nA; ++a) {
-      int s = sums(p, a);
-      double r = pose_response(d, q, s, x, y, a);
-      pm = r > pm ? r : pm;
-      lbest = r > lbest ? r : lbest;
-    }
-    probs[p] = pm;
-  }
-  const double best = block_max(lbest, s_dscratch);
+  uint4 * g4 = reinterpret_cast<uint4 *>(grid);
+  const int n16 = d.data_size / 16;
+  for (int i = threadIdx.x; i < n16; i += blockDim.x) g4[i] = make_uint4(0, 0, 0, 0);
+  for (int i = n16 * 16 + threadIdx.x; i < d.data_size; i += blockDim.x) grid[i] = 0;
+}
 
-  // ordered tie list: poses with DoubleEqual(response, best) in array order (M.cpp:807-817)
-  // each thread owns a contiguous run of cells so that ranks follow array order
-  const int per = (P + blockDim.x - 1) / blockDim.x;
-  const int p0 = min(P, (int)threadIdx.x * per), p1 = min(P, p0 + per);
-  int cnt = 0;
-  for (int p = p0; p < p1; ++p) {
-    const int x = p % d.nX, y = p / d.nX;
-    for (int a = 0; a < nA; ++a)
-      if (double_equal(pose_response(d, q, sums(p, a), x, y, a), best)) ++cnt;
-  }
-  int total = 0;
-  int rank = block_exclusive_scan(cnt, s_iscratch, total);
-  for (int p = p0; p < p1 && rank < kMaxTies; ++p) {
-    const int x = p % d.nX, y = p / d.nX;
-    for (int a = 0; a < nA && rank < kMaxTies; ++a)
-      if (double_equal(pose_response(d, q, sums(p, a), x, y, a), best)) {
-        out.ties[rank++] = p * nA + a;
-      }
-  }
-  __syncthreads();
-  __shared__ double s_avg[2];
-  if (threadIdx.x == 0) {
-    out.best = best;
-    out.best_sum = total > 0 ? sums(out.ties[0] / nA, out.ties[0] % nA) : 0;
-    out.tie_count = total;
-    double ax = 0.0, ay = 0.0;
-    const int m = total < kMaxTies ? total : kMaxTies;
-    for (int t = 0; t < m; ++t) {   // averagePosition += pose position, in order (M.cpp:809)
-      int p = out.ties[t] / nA;
-      ax += d.newx[q * d.nX + p % d.nX];
-      ay += d.newy[q * d.nY + p / d.nX];
-    }
-    if (total > 0) { ax /= total; ay /= total; }
-    s_avg[0] = ax; s_avg[1] = ay;
-    out.avg_x = ax; out.avg_y = ay;
-  }
-  __syncthreads();
-  // positional covariance accumulators (M.cpp:893-933): cells with response >= best - 0.1,
-  // summed in (y, x) order. Terms are formed in parallel, compacted in order, then added
-  // sequentially so the additions happen in the reference's order.
-  const double dx = s_avg[0] - d.center[q * 3 + 0], dy = s_avg[1] - d.center[q * 3 + 1];
-  int c2 = 0;
-  for (int p = p0; p < p1; ++p) if (probs[p] >= (best - 0.1)) ++c2;
-  int tot2 = 0;
-  int r2 = block_exclusive_scan(c2, s_iscratch, tot2);
-  double * terms = probs + P;   // 4 * P doubles of scratch after the probs image
-  for (int p = p0; p < p1; ++p) {
-    double resp = probs[p];
-    if (resp >= (best - 0.1)) {
-      double x = d.xrel[q * d.nX + p % d.nX], y = d.yrel[q * d.nY + p / d.nX];
-      terms[4 * r2 + 0] = resp;
-      terms[4 * r2 + 1] = (square(x - dx) * resp);
-      terms[4 * r2 + 2] = ((x - dx) * (y - dy) * resp);
-      terms[4 * r2 + 3] = (square(y - dy) * resp);
-      ++r2;
+// AddScan's smear (M.cpp:1080-1104) of the valid points of items [it0, it1) into a workspace grid: every tap max-stamps its cell.
+// Cells < 0 are points the order-dependent replay dropped.  half = ksize / 2 and taps = ksize^2 come from the caller, which
+// computes them once per CTA.
+__device__ __forceinline__ void stamp_cells(const SweepDev & d, uint8_t * grid, int it0, int it1, int half, int taps)
+{
+  for (int it = it0; it < it1; ++it) {
+    const int32_t * cl = d.cells + (size_t)it * d.max_n;
+    const int total = d.cell_count[it] * taps;
+    for (int t = threadIdx.x; t < total; t += blockDim.x) {
+      int32_t cell = cl[t / taps];
+      if (cell < 0) continue;
+      const int k = t % taps;
+      uint32_t kv = d.kern[k];
+      if (kv == 0) continue;
+      int gx = (cell & 0xFFFF) + d.roi_x + (k % d.ksize) - half;
+      int gy = (cell >> 16) + d.roi_y + (k / d.ksize) - half;
+      atomic_max_u8(grid + (size_t)gy * d.stride + gx, kv);
     }
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double norm = 0, axx = 0, axy = 0, ayy = 0;
-    for (int t = 0; t < tot2; ++t) {
-      norm += terms[4 * t + 0];
-      axx += terms[4 * t + 1];
-      axy += terms[4 * t + 2];
-      ayy += terms[4 * t + 3];
-    }
-    out.norm = norm; out.acc_xx = axx; out.acc_xy = axy; out.acc_yy = ayy;
-  }
-  __syncthreads();
 }
 
 // Generic fused sweep kernel: one CTA walks pairs p = blockIdx.x, blockIdx.x + gridDim.x, ...
@@ -244,12 +172,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_generic(SweepDev d, int
   for (int pair = blockIdx.x; pair < d.npairs; pair += gridDim.x) {
     const int q = d.pair_query[pair];
     // (1) clear
-    {
-      uint4 * g4 = reinterpret_cast<uint4 *>(grid);
-      const int n16 = d.data_size / 16;
-      for (int i = threadIdx.x; i < n16; i += blockDim.x) g4[i] = make_uint4(0, 0, 0, 0);
-      for (int i = n16 * 16 + threadIdx.x; i < d.data_size; i += blockDim.x) grid[i] = 0;
-    }
+    clear_grid(d, grid);
     if (whole && q != last_q) {
       for (int i = threadIdx.x; i < nA * n; i += blockDim.x) s_off[i] = d.offsets[(size_t)q * nA * n + i];
       last_q = q;
@@ -277,20 +200,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_generic(SweepDev d, int
       }
       __syncthreads();
     }
-    for (int it = it0; it < it1; ++it) {
-      const int32_t * cl = d.cells + (size_t)it * d.max_n;
-      const int total = d.cell_count[it] * taps;
-      for (int t = threadIdx.x; t < total; t += blockDim.x) {
-        int32_t cell = cl[t / taps];
-        if (cell < 0) continue;
-        const int k = t % taps;
-        uint32_t kv = d.kern[k];
-        if (kv == 0) continue;
-        int gx = (cell & 0xFFFF) + d.roi_x + (k % d.ksize) - half;
-        int gy = (cell >> 16) + d.roi_y + (k / d.ksize) - half;
-        atomic_max_u8(grid + (size_t)gy * d.stride + gx, kv);
-      }
-    }
+    stamp_cells(d, grid, it0, it1, half, taps);
     __syncthreads();
     // (3) correlate: items = (angle, pose), angle-major so a warp shares one lookup row; one slice of angles at a time
     const int32_t * pos = d.posidx + (size_t)q * P;
@@ -328,29 +238,11 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_fine(SweepDev d, FineDe
   uint8_t * grid = d.ws_grid + (size_t)blockIdx.x * d.ws_grid_pitch;
   const int half = d.ksize / 2, taps = d.ksize * d.ksize;
   for (int pair = blockIdx.x; pair < d.npairs; pair += gridDim.x) {
-    {
-      uint4 * g4 = reinterpret_cast<uint4 *>(grid);
-      const int n16 = d.data_size / 16;
-      for (int i = threadIdx.x; i < n16; i += blockDim.x) g4[i] = make_uint4(0, 0, 0, 0);
-      for (int i = n16 * 16 + threadIdx.x; i < d.data_size; i += blockDim.x) grid[i] = 0;
-    }
+    clear_grid(d, grid);
     __syncthreads();
     const int it0 = d.pair_item_start[pair], it1 = d.pair_item_start[pair + 1];
     // cells dropped by AddScan's occupancy test were marked < 0 by the coarse pass: plain max-stamp
-    for (int it = it0; it < it1; ++it) {
-      const int32_t * cl = d.cells + (size_t)it * d.max_n;
-      const int total = d.cell_count[it] * taps;
-      for (int t = threadIdx.x; t < total; t += blockDim.x) {
-        int32_t cell = cl[t / taps];
-        if (cell < 0) continue;
-        const int k = t % taps;
-        uint32_t kv = d.kern[k];
-        if (kv == 0) continue;
-        int gx = (cell & 0xFFFF) + d.roi_x + (k % d.ksize) - half;
-        int gy = (cell >> 16) + d.roi_y + (k / d.ksize) - half;
-        atomic_max_u8(grid + (size_t)gy * d.stride + gx, kv);
-      }
-    }
+    stamp_cells(d, grid, it0, it1, half, taps);
     __syncthreads();
     const int P = f.P, nA = f.nA, n = d.n;
     const int32_t * off = f.offsets + (size_t)pair * nA * n;
@@ -373,261 +265,6 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_fine(SweepDev d, FineDe
   }
 }
 
-
-// ------------------------------------------------------------------------------------------
-// Fast sweep kernel (see FastDev in sm_types.cuh).  One CTA (1024 threads, ~224 KB smem) per pair.
-//   smem: S = one parity sub-grid (bytes, row pitch 304 B) | A = int32 accumulators [a][y][x]
-//   per phase (column parity p, row parity q):
-//     raster the taps of every valid point that fall on (p, q) cells into S          (M.cpp:1080-1104)
-//     warp-item = (angle, x-tile of 16 poses); lane = (row y_l = lane / 4, word j_l = lane % 4),
-//       each thread owns rows y_l + 8 r (r < 6) x 4 consecutive x-poses of its word.
-//     for every FAST beam of (angle, phase, alignment m): ONE 32-bit shared load per row gives the
-//       4 poses' grid bytes; two beams' words are added bytewise first (values <= 100, so 2 fit a
-//       byte), then split into 16-bit fields and accumulated; fields are flushed to A every <= 640
-//       beams.  Integer sums are exact, so the volume equals M.cpp:1190-1201 bit for bit.
-//     SLOW beams (window leaves the grid / wraps a row) take the reference's linear-index rule.
-//   then the same reduction as the generic path (pair_epilogue).
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t even_bytes(uint32_t w) { return __byte_perm(w, 0, 0x4240); }   // [b0, 0, b2, 0]
-__device__ __forceinline__ uint32_t odd_bytes(uint32_t w) { return __byte_perm(w, 0, 0x4341); }    // [b1, 0, b3, 0]
-
-__global__ void __launch_bounds__(kFastThreads, 1) k_sweep_fast(SweepDev d, FastDev f)
-{
-  extern __shared__ __align__(16) unsigned char s_raw[];
-  __shared__ double s_dscratch[32];
-  __shared__ int s_iscratch[32];
-  const int sub_words = f.sub_rows * kSubPitchW;
-  uint32_t * S = reinterpret_cast<uint32_t *>(s_raw);
-  uint8_t * S8 = s_raw;
-  int32_t * A = reinterpret_cast<int32_t *>(s_raw + (size_t)sub_words * 4);
-  const int nX = d.nX, nY = d.nY, nA = d.nA, P = nX * nY;
-  const int half = d.ksize / 2, taps = d.ksize * d.ksize;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  const int y_l = lane >> 2, j_l = lane & 3;
-  constexpr int kPitchB = kSubPitchW * 4;
-
-  for (int pair = blockIdx.x; pair < d.npairs; pair += gridDim.x) {
-    const int q = d.pair_query[pair];
-    for (int i = threadIdx.x; i < nA * P; i += blockDim.x) A[i] = 0;
-    const int it0 = d.pair_item_start[pair], it1 = d.pair_item_start[pair + 1];
-
-    for (int ph = 0; ph < 4; ++ph) {
-      const int pp = ph & 1, pq = ph >> 1;
-      __syncthreads();
-      for (int i = threadIdx.x; i < sub_words; i += blockDim.x) S[i] = 0;
-      __syncthreads();
-      // ---- raster: taps landing on (pp, pq) cells ----
-      for (int it = it0; it < it1; ++it) {
-        const int32_t * cl = d.cells + (size_t)it * d.max_n;
-        const int total = d.cell_count[it] * taps;
-        for (int t = threadIdx.x; t < total; t += blockDim.x) {
-          const int32_t cell = cl[t / taps];
-          if (cell < 0) continue;
-          const int k = t % taps;
-          const uint32_t kv = d.kern[k];
-          if (kv == 0) continue;
-          const int gx = (cell & 0xFFFF) + d.roi_x + (k % d.ksize) - half;
-          const int gy = (cell >> 16) + d.roi_y + (k / d.ksize) - half;
-          if ((gx & 1) != pp || (gy & 1) != pq) continue;
-          atomic_max_u8(S8 + (gy >> 1) * kPitchB + (gx >> 1), kv);
-        }
-      }
-      __syncthreads();
-      // ---- FAST beams ----
-      for (int wi = warp; wi < nA * f.xtiles; wi += nwarps) {
-        const int a = wi / f.xtiles, xt = wi - a * f.xtiles;
-        const int32_t * cs = f.cls_start + ((size_t)q * nA + a) * 33 + ph * 8;
-        const int32_t * es = f.edge_start + ((size_t)q * nA + a) * 17 + ph * 4;
-        const uint32_t base = (uint32_t)((y_l * kSubPitchW + 4 * xt + j_l) * 4);
-        int32_t * Arow = A + a * P;
-        for (int m = 0; m < 4; ++m) {
-          // group layout: [plain entries (one per beam) | multi entries (descriptor + multiplicity >= 3)]
-          int b = cs[2 * m];
-          const int mb = cs[2 * m + 1], me = cs[2 * m + 2];
-          bool multi_done = (mb == me);
-          const int x0 = 4 * (4 * xt + j_l) - m;
-          // flush the 16-bit fields: pose x = x0 + t, t = 0..3 (most windows of a sparse grid are empty)
-          auto flush = [&](const uint32_t (&T0)[kFastRowTiles], const uint32_t (&T1)[kFastRowTiles]) {
-            uint32_t any = 0;
-#pragma unroll
-            for (int r = 0; r < kFastRowTiles; ++r) any |= T0[r] | T1[r];
-            if (!__any_sync(0xffffffffu, any != 0)) return;
-#pragma unroll
-            for (int r = 0; r < kFastRowTiles; ++r) {
-              const int y = y_l + 8 * r;
-              if (y >= nY || (T0[r] | T1[r]) == 0) continue;
-              int32_t * dst = Arow + y * nX + x0;
-              const int v0 = T0[r] & 0xFFFF, v1 = T1[r] & 0xFFFF, v2 = T0[r] >> 16, v3 = T1[r] >> 16;
-              if (v0 && (unsigned)(x0 + 0) < (unsigned)nX) atomicAdd(dst + 0, v0);
-              if (v1 && (unsigned)(x0 + 1) < (unsigned)nX) atomicAdd(dst + 1, v1);
-              if (v2 && (unsigned)(x0 + 2) < (unsigned)nX) atomicAdd(dst + 2, v2);
-              if (v3 && (unsigned)(x0 + 3) < (unsigned)nX) atomicAdd(dst + 3, v3);
-            }
-          };
-          do {
-            const int ce = min(mb, b + kFastChunk);
-            uint32_t T0[kFastRowTiles], T1[kFastRowTiles];
-#pragma unroll
-            for (int r = 0; r < kFastRowTiles; ++r) { T0[r] = 0; T1[r] = 0; }
-            // descriptors are fetched 32 at a time (one per lane, coalesced) and broadcast by shuffle
-            for (int b0 = b; b0 < ce; b0 += 32) {
-              const int cnt = min(32, ce - b0);
-              const uint32_t mine = (lane < cnt) ? 4u * f.beams[b0 + lane] : 0u;
-              int k = 0;
-              for (; k + 3 < cnt; k += 4) {   // 4 beams: two byte-wise pair sums, one 3-input add per field
-                const uint32_t o0 = base + __shfl_sync(0xffffffffu, mine, k), o1 = base + __shfl_sync(0xffffffffu, mine, k + 1);
-                const uint32_t o2 = base + __shfl_sync(0xffffffffu, mine, k + 2), o3 = base + __shfl_sync(0xffffffffu, mine, k + 3);
-#pragma unroll
-                for (int r = 0; r < kFastRowTiles; ++r) {
-                  const uint32_t wa = *reinterpret_cast<const uint32_t *>(S8 + o0 + r * 8 * kPitchB) +
-                                      *reinterpret_cast<const uint32_t *>(S8 + o1 + r * 8 * kPitchB);
-                  const uint32_t wb = *reinterpret_cast<const uint32_t *>(S8 + o2 + r * 8 * kPitchB) +
-                                      *reinterpret_cast<const uint32_t *>(S8 + o3 + r * 8 * kPitchB);
-                  T0[r] = T0[r] + even_bytes(wa) + even_bytes(wb);
-                  T1[r] = T1[r] + odd_bytes(wa) + odd_bytes(wb);
-                }
-              }
-              for (; k + 1 < cnt; k += 2) {
-                const uint32_t o0 = base + __shfl_sync(0xffffffffu, mine, k), o1 = base + __shfl_sync(0xffffffffu, mine, k + 1);
-#pragma unroll
-                for (int r = 0; r < kFastRowTiles; ++r) {
-                  const uint32_t w = *reinterpret_cast<const uint32_t *>(S8 + o0 + r * 8 * kPitchB) +
-                                     *reinterpret_cast<const uint32_t *>(S8 + o1 + r * 8 * kPitchB);
-                  T0[r] += even_bytes(w);
-                  T1[r] += odd_bytes(w);
-                }
-              }
-              if (k < cnt) {
-                const uint32_t o0 = base + __shfl_sync(0xffffffffu, mine, k);
-#pragma unroll
-                for (int r = 0; r < kFastRowTiles; ++r) {
-                  const uint32_t w = *reinterpret_cast<const uint32_t *>(S8 + o0 + r * 8 * kPitchB);
-                  T0[r] += even_bytes(w);
-                  T1[r] += odd_bytes(w);
-                }
-              }
-            }
-            b = ce;
-            if (b == mb && !multi_done) {
-              // beams that share one grid cell (several per 5 cm cell at indoor ranges): one load, fields times k.
-              // The host only builds multi entries when the whole group's weight fits one flush (<= kFastChunk).
-              for (int b0 = mb; b0 < me; b0 += 32) {
-                const int cnt = min(32, me - b0);
-                const uint32_t mine = (lane < cnt) ? 4u * f.beams[b0 + lane] : 0u;
-                const uint32_t myk = (lane < cnt) ? f.mult[b0 + lane] : 0u;
-                for (int k = 0; k < cnt; ++k) {
-                  const uint32_t o0 = base + __shfl_sync(0xffffffffu, mine, k);
-                  const uint32_t kk = __shfl_sync(0xffffffffu, myk, k);
-#pragma unroll
-                  for (int r = 0; r < kFastRowTiles; ++r) {
-                    const uint32_t w = *reinterpret_cast<const uint32_t *>(S8 + o0 + r * 8 * kPitchB);
-                    T0[r] += even_bytes(w) * kk;
-                    T1[r] += odd_bytes(w) * kk;
-                  }
-                }
-              }
-              multi_done = true;
-            }
-            flush(T0, T1);
-          } while (b < mb || !multi_done);
-          // EDGE beams of this group (window partly outside the grid): same word loads, but rows / words that fall
-          // outside the sub-grid are skipped (they index outside [0, data_size) or wrap in the reference; the wrapped
-          // part is added by the secondary list below). Rows / words inside the allocation but beyond the valid cells
-          // are zero padding, so only the allocation bounds need checking.
-          int eb = es[m];
-          const int ee = es[m + 1];
-          while (eb < ee) {
-            const int ce = min(ee, eb + kFastChunk);
-            uint32_t T0[kFastRowTiles], T1[kFastRowTiles];
-#pragma unroll
-            for (int r = 0; r < kFastRowTiles; ++r) { T0[r] = 0; T1[r] = 0; }
-            for (int b0 = eb; b0 < ce; b0 += 32) {
-              const int cnt = min(32, ce - b0);
-              const int32_t mine = (lane < cnt) ? f.edge[b0 + lane] : 0;
-              for (int k = 0; k < cnt; ++k) {
-                const int32_t e = __shfl_sync(0xffffffffu, mine, k);
-                const int row0 = (int)(int16_t)(e & 0xFFFF) + y_l, wq = (e >> 16) + 4 * xt + j_l;
-                const bool cv = (unsigned)wq < (unsigned)kSubPitchW;
-#pragma unroll
-                for (int r = 0; r < kFastRowTiles; ++r) {
-                  const int row = row0 + 8 * r;
-                  const uint32_t w = (cv && (unsigned)row < (unsigned)f.sub_rows) ? S[row * kSubPitchW + wq] : 0u;
-                  T0[r] += even_bytes(w);
-                  T1[r] += odd_bytes(w);
-                }
-              }
-            }
-            eb = ce;
-            flush(T0, T1);
-          }
-        }
-      }
-      // ---- EDGE beams: the window leaves the grid (readings close to / beyond the range threshold).
-      //   primary list (this phase = the beam's own parity): poses whose column stays inside [0, stride); rows outside
-      //     [0, height) index outside [0, data_size) in the reference and contribute 0;
-      //   secondary list (row parity flipped): poses whose column left [0, stride) by less than one stride -- the
-      //     reference's linear index (M.cpp:1192-1200) makes them read the neighbouring row at column -/+ stride.
-      //   Every thread owns up to 3 fixed poses (coordinates in registers: no division in the loops) and walks the beams. ----
-      {
-        const bool has_wrap = f.wrap2_start[((size_t)q * nA + nA - 1) * 4 + 4] - f.wrap2_start[(size_t)q * nA * 4] > 0;
-        if (has_wrap) {
-          int ex[3], ey[3];
-#pragma unroll
-          for (int k = 0; k < 3; ++k) {
-            const int p = threadIdx.x + k * kFastThreads;
-            ex[k] = p < P ? 2 * (p % nX) : -100000;   // poses beyond P never hit a valid column
-            ey[k] = 2 * (p / nX);
-          }
-          if (has_wrap) {
-            const int32_t * cl = f.wrap2_start + ((size_t)q * nA) * 4 + ph;
-            for (int a = 0; a < nA; ++a) {
-              int32_t * Aa = A + a * P + threadIdx.x;
-              for (int bi = cl[4 * a]; bi < cl[4 * a + 1]; ++bi) {
-                const int32_t e = f.wrap2[bi];
-                const int Xb = (int)(int16_t)(e & 0xFFFF), Yb = e >> 16;
-#pragma unroll
-                for (int k = 0; k < 3; ++k) {
-                  const int col = Xb + ex[k];
-                  if ((unsigned)col < (unsigned)d.stride || ex[k] < 0) continue;
-                  const int r2 = Yb + ey[k] + (col < 0 ? -1 : 1);
-                  const int c2 = col + (col < 0 ? d.stride : -d.stride);
-                  if ((unsigned)r2 >= (unsigned)d.height) continue;
-                  const int v = S8[(r2 >> 1) * kPitchB + (c2 >> 1)];
-                  if (v) atomicAdd(Aa + k * kFastThreads, v);
-                }
-              }
-            }
-          }
-        }
-      }
-      // ---- FAR beams: column offsets of a stride or more (readings near the laser's maximum range at fine grids):
-      //      pose by pose on the linear index with a division, every phase. Rare. ----
-      {
-        const int32_t * ss = f.slow_start + (size_t)q * (nA + 1);
-        const int nslow = ss[nA] - ss[0];
-        if (nslow > 0) {
-          const int32_t * pos = d.posidx + (size_t)q * P;
-          for (int a = 0; a < nA; ++a) {
-            const int sb = ss[a], se = ss[a + 1];
-            const int work = (se - sb) * P;
-            for (int t = threadIdx.x; t < work; t += blockDim.x) {
-              const int bi = t / P, p = t - bi * P;
-              const int idx = pos[p] + f.slow[sb + bi];
-              if ((unsigned)idx >= (unsigned)d.data_size) continue;
-              const int row = idx / d.stride, col = idx - row * d.stride;
-              if ((col & 1) != pp || (row & 1) != pq) continue;
-              const int v = S8[(row >> 1) * kPitchB + (col >> 1)];
-              if (v) atomicAdd(A + a * P + p, v);
-            }
-          }
-        }
-      }
-    }
-    __syncthreads();
-    // S is free now: reuse it as the FP64 scratch of the reduction (5 P doubles)
-    pair_epilogue(d, pair, q, SumsAngleMajor{A, P}, reinterpret_cast<double *>(s_raw), s_dscratch, s_iscratch);
-  }
-}
 
 // Per-query best-response key for the multi-GPU sweep: key = best_sum << 32 | (0xFFFFFFFF - global
 // candidate id), so that a max-reduction (here atomicMax, across GPUs ncclMax) picks the highest
@@ -727,13 +364,6 @@ void sweep_stage_h2d(void * dst, const void * src, size_t bytes, cudaStream_t s)
   if (g_h2d_counter) *g_h2d_counter += (int64_t)bytes;
 }
 
-template <class T>
-static void h2d(DevBuf<T> & dst, const T * src, size_t count, cudaStream_t s)
-{
-  dst.reserve(count);
-  sweep_stage_h2d(dst.p, src, count * sizeof(T), s);
-}
-
 static GridGeom geom_for_query(const b200sm * h, const b200_scan * q)
 {
   GridGeom g;
@@ -753,7 +383,6 @@ static void coarse_search(const b200sm * h, double off[2], double res[2])
   res[0] = res[1] = 2 * r;                 // M.cpp:584-585
 }
 
-static bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st);
 
 // shared memory the generic kernel may fill with lookup rows; a query needs at least one row (n <= 51,200 readings)
 constexpr size_t kGenericTableBytes = 200 * 1024;
@@ -773,7 +402,15 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   const auto t_enter = std::chrono::steady_clock::now();
   SweepHost & S = h->sweep;
   S.uploaded = S.ran = false;
-  S.zero_done.clear(); S.zero_exp_done.clear();
+  S.zero.done.clear(); S.zero_exp.done.clear();
+  // readouts of the kernel choice: the builder that succeeds fills in its own.  The builders' refusal codes (tile_info[5],
+  // fast_refusal) stay until that builder runs again.
+  S.kernel = kSweepGeneric; S.refused_reason = 0;
+  S.fast.enabled = 0; S.tile.enabled = 0;
+  std::fill(S.beam_counts, S.beam_counts + 3, 0);
+  for (int i = 0; i < 8; ++i) if (i != 5) S.tile_info[i] = 0;
+  std::fill(S.tile_stats, S.tile_stats + 8, 0);
+  std::fill(S.tile_layout, S.tile_layout + 4, 0);
   g_h2d_counter = &S.h2d_bytes;
   if (!queries || nq <= 0 || !scans || nscans <= 0 || !chain_start || nchains <= 0) {
     set_last_error("sweep: empty or NULL input");
@@ -971,192 +608,23 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   d.ws_probs = S.d_ws_probs.p; d.ws_probs_pitch = ppitch;
   d.out = S.d_out.p;
   if (!S.ev0) { B200_CUDA(cudaEventCreate(&S.ev0)); B200_CUDA(cudaEventCreate(&S.ev1)); }
-  // tables of the kernel that will run only (see sweep_kernel_choice).  The tiled cluster kernel is the default everywhere: with
-  // the atomic-free levelled raster it is ahead of the single-CTA kernel on that kernel's own geometry too (on an H100, 400 W power
-  // limit: 387 k vs 273 k matches/s at cfg2, bench.py); "sweep_kernel" = 1 still selects the single-CTA kernel.
-  S.fast.enabled = 0; S.tile.enabled = 0;
-  S.fast_info[0] = 0; S.tile_info[0] = 0;
-  for (int i = 0; i < 4; ++i) S.tile_layout[i] = 0;
+  // The kernel is chosen here, once, and only its tables are built: the tiled cluster kernel (any geometry with an even stride and
+  // an order-independent raster) is the default everywhere.  With the atomic-free levelled raster it is ahead of the single-CTA
+  // kernel on that kernel's own geometry too (on an H100, 400 W power limit: 387 k vs 273 k matches/s at cfg2, bench.py); the
+  // single-CTA kernel takes what the tiled planner refuses, and "sweep_kernel" = 1 selects it first.  Anything else runs on the
+  // generic kernel.
   const auto t_tab0 = std::chrono::steady_clock::now();
-  bool have = false;
-  if (!h->force_generic && h->sweep_kernel == 1) have = build_fast_tables(h, S, st);
-  if (!h->force_generic && !have) have = build_tile_tables(h, S, st);
-  if (!h->force_generic && !have && h->sweep_kernel != 1) build_fast_tables(h, S, st);
+  if (!h->force_generic) {
+    if (h->sweep_kernel == 1 && build_fast_tables(h, S, st)) S.kernel = kSweepFast;
+    else if (build_tile_tables(h, S, st)) S.kernel = kSweepTile;
+    else if (h->sweep_kernel != 1 && build_fast_tables(h, S, st)) S.kernel = kSweepFast;
+    else S.refused_reason = S.tile_info[5] ? 100 + S.tile_info[5] : S.fast_refusal;
+  }
   const auto t_tab1 = std::chrono::steady_clock::now();
   auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
   S.upload_ms[0] = ms(t_plans0, t_plans1); S.upload_ms[1] = ms(t_tab0, t_tab1); S.upload_ms[2] = ms(t_enter, t_tab1);
   S.uploaded = true;
   return B200_OK;
-}
-
-// Builds the per-query beam lists of the fast path; returns false when this sweep cannot use it.
-static bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st)
-{
-  const GridGeom & g = h->g;
-  const CorrPlan & p0 = S.plans[0];
-  const int nX = p0.nX, nY = p0.nY, nA = p0.nA, n = p0.n, nq = S.nq;
-  S.fast.enabled = 0;
-  S.fast_info[0] = 0; S.fast_info[1] = S.fast_info[2] = S.fast_info[3] = 0;
-  auto bail = [&](int why) { S.fast_info[4] = why; return false; };
-  if (g.order_dependent) return bail(1);
-  if (nY > 8 * kFastRowTiles || (g.stride & 1) || nX * nY > 3 * kFastThreads) return bail(2);
-  if (g.stride / 2 > kSubPitchW * 4 - 16) return bail(3);   // sub-grid row + the 3-word overhang must fit the pitch
-  const int xtiles = (nX + 3 + 15) / 16;
-  int sub_rows = (g.height + 1) / 2 + 8;                     // + padding rows read by idle row tiles
-  // the S region doubles as the FP64 scratch of the reduction (5 P doubles): small grids get extra rows for it
-  sub_rows = std::max(sub_rows, (int)(((size_t)5 * nX * nY * sizeof(double) + kSubPitchW * 4 - 1) / (kSubPitchW * 4)));
-  const size_t smem = (size_t)sub_rows * kSubPitchW * 4 + (size_t)nA * nX * nY * 4;
-  if (smem > 227 * 1024 - 1024) return bail(4);
-  if ((size_t)5 * nX * nY * sizeof(double) > (size_t)sub_rows * kSubPitchW * 4) return bail(5);   // epilogue scratch reuses S
-  std::vector<int32_t> cls_start((size_t)nq * nA * 33), slow, slow_start((size_t)nq * (nA + 1));
-  std::vector<uint16_t> beams, mult;
-  std::vector<int32_t> wrap2, wrap2_start((size_t)nq * nA * 4 + 1);
-  std::vector<int32_t> edge, edge_start((size_t)nq * nA * 17);
-  int n_edge = 0;
-  beams.reserve((size_t)nq * nA * n);
-  mult.reserve((size_t)nq * nA * n);
-  // one angle's lists, built independently (one host-pool task per angle), then concatenated in angle order
-  struct AngleLists {
-    std::vector<uint16_t> beams, mult;
-    int32_t cs[33];                          // relative to the angle's first descriptor
-    std::vector<int32_t> wgroup[4], egroup[16], slow;
-    int n_edge = 0;
-  };
-  std::vector<AngleLists> al(nA);
-  for (int q = 0; q < nq; ++q) {
-    const CorrPlan & pl = S.plans[q];
-    for (int k = 1; k < nX; ++k) if (pl.xs[k] != pl.xs[0] + 2 * k) return bail(6);   // coarse step must be exactly 2 cells
-    for (int k = 1; k < nY; ++k) if (pl.ys[k] != pl.ys[0] + 2 * k) return bail(7);
-    const int X0 = pl.xs[0], Y0 = pl.ys[0];
-    auto one_angle = [&](int a) {
-      AngleLists & L = al[a];
-      std::vector<uint16_t> group[16];
-      L.beams.clear(); L.mult.clear(); L.slow.clear(); L.n_edge = 0;
-      for (auto & v : L.wgroup) v.clear();
-      for (auto & v : L.egroup) v.clear();
-      for (int i = 0; i < n; ++i) {
-        const int32_t off = pl.offsets[(size_t)a * n + i];
-        if (off == kInvalidScan) continue;
-        const int gx = pl.ogx[(size_t)a * n + i], gy = pl.ogy[(size_t)a * n + i];
-        const int Xb = X0 + gx, Yb = Y0 + gy;
-        const bool inside = Xb >= 0 && Xb + 2 * (nX - 1) < g.stride && Yb >= 0 && Yb + 2 * (nY - 1) < g.height;
-        if (inside) {
-          const int pp = Xb & 1, pq = Yb & 1, c = Xb >> 1, r = Yb >> 1;
-          const int wo = r * kSubPitchW + (c >> 2);
-          group[(pq * 2 + pp) * 4 + (c & 3)].push_back((uint16_t)wo);
-        } else if (Xb >= -g.stride && Xb + 2 * (nX - 1) < 2 * g.stride && Xb > -32768 && Xb < 32767 && Yb > -32768 && Yb < 32767) {
-          // EDGE beam: at most one row wrap. Primary entry in the beam's own phase; if some column leaves
-          // [0, stride), a secondary entry in the phase with the row parity flipped.
-          const int32_t e = (int32_t)((uint32_t)(Xb & 0xFFFF) | ((uint32_t)Yb << 16));
-          const bool rows_hit = Yb + 2 * (nY - 1) >= 0 && Yb < g.height;
-          const bool cols_hit = Xb + 2 * (nX - 1) >= 0 && Xb < g.stride;
-          if (rows_hit && cols_hit) {
-            const int c = Xb >> 1, r = Yb >> 1;   // arithmetic shifts: floor for negative coordinates
-            L.egroup[((Yb & 1) * 2 + (Xb & 1)) * 4 + (c & 3)].push_back((int32_t)((uint32_t)(r & 0xFFFF) | ((uint32_t)(c >> 2) << 16)));
-            ++L.n_edge;
-          }
-          const bool wraps = Xb < 0 || Xb + 2 * (nX - 1) >= g.stride;
-          if (wraps && Yb + 2 * (nY - 1) + 1 >= 0 && Yb - 1 < g.height) L.wgroup[((Yb & 1) ^ 1) * 2 + (Xb & 1)].push_back(e);
-        } else {
-          const int32_t dv = device_offset(off, g.data_size);
-          if (dv != kDevInvalid) L.slow.push_back(dv);   // FAR: can still index [0, data_size) for some pose
-        }
-      }
-      for (int k = 0; k < 16; ++k) {
-        std::vector<uint16_t> & gk = group[k];
-        std::sort(gk.begin(), gk.end());
-        L.cs[2 * k] = (int32_t)L.beams.size();
-        // run-length encode: beams that land in the same cell share a descriptor. Entries with multiplicity >= 3
-        // go to the group's multi list (one load, fields multiplied), provided the whole group fits one flush.
-        const bool dedup = !h->no_dedup && gk.size() <= (size_t)kFastChunk;
-        std::vector<std::pair<uint16_t, uint16_t>> multi;
-        for (size_t i = 0; i < gk.size();) {
-          size_t j = i;
-          while (j < gk.size() && gk[j] == gk[i]) ++j;
-          const size_t cnt = j - i;
-          if (dedup && cnt >= 3) {
-            multi.emplace_back(gk[i], (uint16_t)cnt);
-          } else {
-            for (size_t t = 0; t < cnt; ++t) { L.beams.push_back(gk[i]); L.mult.push_back(1); }
-          }
-          i = j;
-        }
-        L.cs[2 * k + 1] = (int32_t)L.beams.size();
-        for (auto & mk : multi) { L.beams.push_back(mk.first); L.mult.push_back(mk.second); }
-      }
-      L.cs[32] = (int32_t)L.beams.size();
-    };
-    host_parallel_for(nA, one_angle);
-    for (int a = 0; a < nA; ++a) {
-      const AngleLists & L = al[a];
-      slow_start[(size_t)q * (nA + 1) + a] = (int32_t)slow.size();
-      slow.insert(slow.end(), L.slow.begin(), L.slow.end());
-      n_edge += L.n_edge;
-      for (int k = 0; k < 4; ++k) {
-        wrap2_start[((size_t)q * nA + a) * 4 + k] = (int32_t)wrap2.size();
-        wrap2.insert(wrap2.end(), L.wgroup[k].begin(), L.wgroup[k].end());
-      }
-      for (int k = 0; k < 16; ++k) {
-        edge_start[((size_t)q * nA + a) * 17 + k] = (int32_t)edge.size();
-        edge.insert(edge.end(), L.egroup[k].begin(), L.egroup[k].end());
-      }
-      edge_start[((size_t)q * nA + a) * 17 + 16] = (int32_t)edge.size();
-      int32_t * cs = &cls_start[((size_t)q * nA + a) * 33];
-      const int32_t base = (int32_t)beams.size();
-      for (int k = 0; k < 33; ++k) cs[k] = base + L.cs[k];
-      beams.insert(beams.end(), L.beams.begin(), L.beams.end());
-      mult.insert(mult.end(), L.mult.begin(), L.mult.end());
-    }
-    slow_start[(size_t)q * (nA + 1) + nA] = (int32_t)slow.size();
-  }
-  wrap2_start[(size_t)nq * nA * 4] = (int32_t)wrap2.size();
-  // slow_start must be relative to one array: it is (single vector `slow`)
-  h2d(S.d_fast_cls, cls_start.data(), cls_start.size(), st);
-  S.d_fast_beams.reserve(std::max<size_t>(beams.size(), 1) + 8);
-  sweep_stage_h2d(S.d_fast_beams.p, beams.data(), beams.size() * sizeof(uint16_t), st);
-  S.d_fast_mult.reserve(std::max<size_t>(mult.size(), 1) + 8);
-  sweep_stage_h2d(S.d_fast_mult.p, mult.data(), mult.size() * sizeof(uint16_t), st);
-  slow.push_back(0);
-  wrap2.push_back(0);
-  edge.push_back(0);
-  h2d(S.d_fast_edge, edge.data(), edge.size(), st);
-  h2d(S.d_fast_edge_start, edge_start.data(), edge_start.size(), st);
-  h2d(S.d_fast_wrap2, wrap2.data(), wrap2.size(), st);
-  h2d(S.d_fast_wrap2_start, wrap2_start.data(), wrap2_start.size(), st);
-  h2d(S.d_fast_slow, slow.data(), slow.size(), st);
-  h2d(S.d_fast_slow_start, slow_start.data(), slow_start.size(), st);
-  S.fast.enabled = 1;
-  S.fast_info[0] = 1; S.fast_info[1] = (int32_t)beams.size(); S.fast_info[2] = n_edge; S.fast_info[3] = (int32_t)slow.size() - 1; S.fast_info[4] = 0;
-  S.fast.sub_rows = sub_rows;
-  S.fast.xtiles = xtiles;
-  S.fast.beams = S.d_fast_beams.p;
-  S.fast.mult = S.d_fast_mult.p;
-  S.fast.cls_start = S.d_fast_cls.p;
-  S.fast.slow = S.d_fast_slow.p;
-  S.fast.edge = S.d_fast_edge.p;
-  S.fast.edge_start = S.d_fast_edge_start.p;
-  S.fast.wrap2 = S.d_fast_wrap2.p;
-  S.fast.wrap2_start = S.d_fast_wrap2_start.p;
-  S.fast.slow_start = S.d_fast_slow_start.p;
-  S.fast_smem = smem;
-  {
-    int dev = 0, sms = 132;
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    S.fast_blocks = std::min(S.npairs, sms);
-  }
-  return true;
-}
-
-// which kernel an uploaded sweep runs on: 0 = generic (any geometry), 1 = single-CTA fast kernel (BASELINE's 4 m / 12 m
-// geometry), 2 = tiled cluster kernel (any even-stride geometry whose raster is order independent)
-static int sweep_kernel_choice(const b200sm * h, const SweepHost & S)
-{
-  if (h->force_generic) return 0;
-  const bool fast = S.fast.enabled != 0, tile = S.tile.enabled != 0;
-  if (h->sweep_kernel == 1 && fast) return 1;
-  if (tile) return 2;
-  return fast ? 1 : 0;
 }
 
 static int sweep_run(b200sm * h)
@@ -1177,13 +645,13 @@ static int sweep_run(b200sm * h)
     h->launches++;
   }
   B200_CUDA(cudaEventRecord(S.ev0, st));
-  switch (sweep_kernel_choice(h, S)) {
-    case 2:
-      launch_sweep_tile(h, S, st);
+  // "force_generic_sweep" set after the upload still takes effect: the generic kernel needs no tables of its own
+  switch (h->force_generic ? kSweepGeneric : S.kernel) {
+    case kSweepTile:
+      launch_sweep_tile(S, st);
       break;
-    case 1:
-      B200_CUDA(cudaFuncSetAttribute(k_sweep_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S.fast_smem));
-      k_sweep_fast<<<S.fast_blocks, kFastThreads, S.fast_smem, st>>>(d, S.fast);
+    case kSweepFast:
+      launch_sweep_fast(S, st);
       break;
     default: {
       const int rows = generic_slice_rows(d.nA, d.n);
@@ -1221,6 +689,20 @@ static void zero_volume_result(const CorrPlan & pl, double mean[3], double cov[9
   cov[0] = kMaxVariance; cov[4] = kMaxVariance; cov[8] = 4 * square(pl.ang_res);
 }
 
+// Copies query q's entry of the cache to mean / cov, evaluating it first with compute(mean, cov) (false: it cannot be evaluated)
+template <class F>
+static bool cached_zero_result(ZeroCache & c, int nq, int q, F compute, double * mean, double * cov)
+{
+  if ((int)c.done.size() != nq) { c.done.assign(nq, 0); c.mean.assign((size_t)3 * nq, 0.0); c.cov.assign((size_t)9 * nq, 0.0); }
+  if (!c.done[q]) {
+    if (!compute(&c.mean[3 * (size_t)q], &c.cov[9 * (size_t)q])) return false;
+    c.done[q] = 1;
+  }
+  for (int i = 0; i < 3; ++i) mean[i] = c.mean[3 * (size_t)q + i];
+  for (int i = 0; i < 9; ++i) cov[i] = c.cov[9 * (size_t)q + i];
+  return true;
+}
+
 // finish one pair on the host from the device reduction: heading average (libm) + covariance tail
 // raster_empty: 1 = no valid point of the pair's chain fell inside the correlation grid (every lookup of every pass is 0),
 // 0 = some did, -1 = unknown
@@ -1232,8 +714,7 @@ static bool finish_query_pair(const b200sm * h, SweepHost & S, int q, const Pair
     // M.cpp:594-619: up to three more coarse passes with the angle window widened by 20 degrees each.  With an EMPTY raster all
     // of them are zero too, so the result is the all-poses-tie average of the last (widest) pass: closed form, once per query.
     if (raster_empty != 1) return false;   // cells exist: a wider pass could hit them -> single-match path
-    if ((int)S.zero_exp_done.size() != S.nq) { S.zero_exp_done.assign(S.nq, 0); S.zero_exp_mean.assign((size_t)3 * S.nq, 0.0); S.zero_exp_cov.assign((size_t)9 * S.nq, 0.0); }
-    if (!S.zero_exp_done[q]) {
+    auto widest = [&](double * m, double * c) {
       double off[2], res[2];
       coarse_search(h, off, res);
       GridGeom g = geom_for_query(h, &S.queries[q]);
@@ -1242,20 +723,16 @@ static bool finish_query_pair(const b200sm * h, SweepHost & S, int q, const Pair
       CorrPlan px;
       if (build_plan(g, h->probs_side, h->p, &S.queries[q], S.queries[q].sensor_pose, off, res, wide, h->p.coarse_angle_resolution, false, px) != B200_OK)
         return false;
-      zero_volume_result(px, &S.zero_exp_mean[3 * (size_t)q], &S.zero_exp_cov[9 * (size_t)q]);
-      S.zero_exp_done[q] = 1;
-    }
-    for (int i = 0; i < 3; ++i) mean[i] = S.zero_exp_mean[3 * (size_t)q + i];
-    for (int i = 0; i < 9; ++i) cov[i] = S.zero_exp_cov[9 * (size_t)q + i];
+      zero_volume_result(px, m, c);
+      return true;
+    };
+    if (!cached_zero_result(S.zero_exp, S.nq, q, widest, mean, cov)) return false;
     *response = 0.0;
     S.zero_pairs++;
     return true;
   }
   if (o.best == 0.0 && o.tie_count == pl.nX * pl.nY * pl.nA && o.tie_count > kMaxTies) {
-    if ((int)S.zero_done.size() != S.nq) { S.zero_done.assign(S.nq, 0); S.zero_mean.assign((size_t)3 * S.nq, 0.0); S.zero_cov.assign((size_t)9 * S.nq, 0.0); }
-    if (!S.zero_done[q]) { zero_volume_result(pl, &S.zero_mean[3 * (size_t)q], &S.zero_cov[9 * (size_t)q]); S.zero_done[q] = 1; }
-    for (int i = 0; i < 3; ++i) mean[i] = S.zero_mean[3 * (size_t)q + i];
-    for (int i = 0; i < 9; ++i) cov[i] = S.zero_cov[9 * (size_t)q + i];
+    cached_zero_result(S.zero, S.nq, q, [&](double * m, double * c) { zero_volume_result(pl, m, c); return true; }, mean, cov);
     *response = 0.0;
     S.zero_pairs++;
     return true;
@@ -1539,11 +1016,10 @@ int b200sm_batch_info(b200sm * h, int32_t info[8])
 {
   if (!h || !info || !h->sweep.uploaded) return B200_ERR_INVALID_ARG;
   const SweepHost & S = h->sweep;
-  const int k = sweep_kernel_choice(h, S);
-  for (int i = 0; i < 5; ++i) info[i] = S.fast_info[i];
-  info[0] = k;
-  if (k == 2) info[4] = 0; else if (k == 0 && S.tile_info[5]) info[4] = 100 + S.tile_info[5];
-  info[5] = k == 2 ? S.tile_grid : (k == 1 ? S.fast_blocks : S.blocks);
+  info[0] = S.kernel;
+  for (int i = 0; i < 3; ++i) info[1 + i] = S.beam_counts[i];
+  info[4] = S.refused_reason;
+  info[5] = S.kernel == kSweepTile ? S.tile_grid : (S.kernel == kSweepFast ? S.fast_blocks : S.blocks);
   info[6] = S.npairs; info[7] = S.nitems;
   return B200_OK;
 }

@@ -4,7 +4,7 @@
 // (lib/karto_sdk/src/Mapper.cpp:534-1208, "M.cpp"), called once per candidate chain by
 // MapperGraph::TryCloseLoop (M.cpp:1500-1561).
 //
-// k_sweep_fast (sm_sweep.cu) keeps one parity sub-grid and the whole (x, y, theta) accumulator volume of
+// k_sweep_fast (sm_fast.cu) keeps one parity sub-grid and the whole (x, y, theta) accumulator volume of
 // a pair in ONE SM's shared memory, which only holds for BASELINE's 4 m / 12 m geometry.  This kernel lifts
 // both limits so that the reference's shipped geometries (loop_search_space_dimension 8 m -> 81 x 81 x 21
 // poses = 551 KB of accumulators; max_laser_range 20 m -> 881..965-cell grids) run on the same word-load
@@ -29,7 +29,6 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -908,6 +907,59 @@ static bool build_block_items(const std::vector<int32_t> & tbl, const std::vecto
   return true;
 }
 
+void classify_beams(const GridGeom & g, const CorrPlan & pl, int a, int pitch_w, int band_rows, int nbands, BeamClasses & c)
+{
+  const int nX = pl.nX, nY = pl.nY, n = pl.n, nstage = 4 * nbands, B = band_rows;
+  const int X0 = pl.xs[0], Y0 = pl.ys[0];
+  c.fast.resize((size_t)nstage * 4);
+  c.edge.resize((size_t)nstage * 4);
+  c.wrap2.resize(nstage);
+  for (auto & v : c.fast) v.clear();
+  for (auto & v : c.edge) v.clear();
+  for (auto & v : c.wrap2) v.clear();
+  c.far.clear();
+  int nf = 0, ne = 0;
+  for (int i = 0; i < n; ++i) {
+    const int32_t off = pl.offsets[(size_t)a * n + i];
+    if (off == kInvalidScan) continue;
+    const int gx = pl.ogx[(size_t)a * n + i], gy = pl.ogy[(size_t)a * n + i];
+    const int Xb = X0 + gx, Yb = Y0 + gy;
+    const bool inside = Xb >= 0 && Xb + 2 * (nX - 1) < g.stride && Yb >= 0 && Yb + 2 * (nY - 1) < g.height;
+    if (inside) {
+      const int pp = Xb & 1, pq = Yb & 1, cx = Xb >> 1, r = Yb >> 1;
+      const int band = std::min(r / B, nbands - 1);
+      const int wo = (r - band * B) * pitch_w + (cx >> 2);
+      c.fast[((pq * 2 + pp) * nbands + band) * 4 + (cx & 3)].push_back((uint16_t)wo);
+      ++nf;
+    } else if (Xb >= -g.stride && Xb + 2 * (nX - 1) < 2 * g.stride && Xb > -32768 && Xb < 32767 && Yb > -32768 && Yb < 32767) {
+      // EDGE beam: at most one row wrap.  Primary entry in the beam's own phase; if some column leaves [0, stride), a
+      // secondary entry in the phase with the row parity flipped.
+      const bool rows_hit = Yb + 2 * (nY - 1) >= 0 && Yb < g.height;
+      const bool cols_hit = Xb + 2 * (nX - 1) >= 0 && Xb < g.stride;
+      if (rows_hit && cols_hit) {
+        const int cx = Xb >> 1, r = Yb >> 1;   // arithmetic shifts: floor for negative coordinates
+        const int band = std::min(std::max(floor_div(r, B), 0), nbands - 1);
+        const int rr = r - band * B;
+        if (rr > -32768 && rr < 32767) {
+          c.edge[(((Yb & 1) * 2 + (Xb & 1)) * nbands + band) * 4 + (cx & 3)].push_back(
+            (int32_t)((uint32_t)(rr & 0xFFFF) | ((uint32_t)(cx >> 2) << 16)));
+          ++ne;
+        }
+      }
+      const bool wraps = Xb < 0 || Xb + 2 * (nX - 1) >= g.stride;
+      if (wraps && Yb + 2 * (nY - 1) + 1 >= 0 && Yb - 1 < g.height) {
+        const int r = (Yb - 1) >> 1;
+        const int band = std::min(std::max(floor_div(r, B), 0), nbands - 1);
+        c.wrap2[(((Yb & 1) ^ 1) * 2 + (Xb & 1)) * nbands + band].push_back((int32_t)((uint32_t)(Xb & 0xFFFF) | ((uint32_t)Yb << 16)));
+      }
+    } else {
+      const int32_t dv = device_offset(off, g.data_size);
+      if (dv != kDevInvalid) c.far.push_back(dv);   // FAR: can still index [0, data_size) for some pose
+    }
+  }
+  c.n_fast = nf; c.n_edge = ne;
+}
+
 bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
 {
   const GridGeom & g = h->g;
@@ -915,9 +967,6 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   const int nX = p0.nX, nY = p0.nY, nA = p0.nA, n = p0.n, nq = S.nq, P = nX * nY;
   TileDev & T = S.tile;
   T = TileDev{};
-  for (int i = 0; i < 8; ++i) S.tile_info[i] = 0;
-  for (int i = 0; i < 4; ++i) S.tile_layout[i] = 0;
-  for (int i = 0; i < 8; ++i) S.tile_stats[i] = 0;
   auto bail = [&](int why) {
     for (int i = 0; i < 8; ++i) S.tile_stats[i] = 0;
     S.tile_info[5] = why;
@@ -1056,62 +1105,15 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   std::vector<int32_t> wrap2, wrap2_start((size_t)nq * nA * nstage + 1, 0);
   std::vector<int32_t> slow, slow_start((size_t)nq * (nA + 1), 0);
   int n_fast = 0, n_edge = 0;
-  std::vector<std::vector<uint16_t>> grp((size_t)nA * nstage * 4);
-  std::vector<std::vector<int32_t>> egrp((size_t)nA * nstage * 4), wgrp((size_t)nA * nstage);
+  std::vector<BeamClasses> cls(nA);
   blob.reserve((size_t)nq * nA * n * 2 + 4096);
   struct Encoded { int32_t tbl[16]; std::vector<uint16_t> pay; };
   std::vector<Encoded> enc((size_t)nA * nstage);
-  std::vector<std::vector<int32_t>> slow_a(nA);
-  std::vector<int> nfast_a(nA), nedge_a(nA);
   for (int q = 0; q < nq; ++q) {
     const CorrPlan & pl = S.plans[q];
-    const int X0 = pl.xs[0], Y0 = pl.ys[0];
     // one host-pool task per angle: classify its beams, then sort / run-length encode its groups stage by stage
     auto one_angle = [&](int a) {
-      for (int k = 0; k < nstage * 4; ++k) { grp[(size_t)a * nstage * 4 + k].clear(); egrp[(size_t)a * nstage * 4 + k].clear(); }
-      for (int k = 0; k < nstage; ++k) wgrp[(size_t)a * nstage + k].clear();
-      slow_a[a].clear();
-      int nf = 0, ne = 0;
-      for (int i = 0; i < n; ++i) {
-        const int32_t off = pl.offsets[(size_t)a * n + i];
-        if (off == kInvalidScan) continue;
-        const int gx = pl.ogx[(size_t)a * n + i], gy = pl.ogy[(size_t)a * n + i];
-        const int Xb = X0 + gx, Yb = Y0 + gy;
-        const bool inside = Xb >= 0 && Xb + 2 * (nX - 1) < g.stride && Yb >= 0 && Yb + 2 * (nY - 1) < g.height;
-        if (inside) {
-          const int pp = Xb & 1, pq = Yb & 1, c = Xb >> 1, r = Yb >> 1;
-          const int band = std::min(r / B, nbands - 1);
-          const int wo = (r - band * B) * pitch_w + (c >> 2);
-          grp[((size_t)a * nstage + (pq * 2 + pp) * nbands + band) * 4 + (c & 3)].push_back((uint16_t)wo);
-          ++nf;
-        } else if (Xb >= -g.stride && Xb + 2 * (nX - 1) < 2 * g.stride && Xb > -32768 && Xb < 32767 && Yb > -32768 && Yb < 32767) {
-          // EDGE beam: at most one row wrap.  Primary entry in the beam's own phase; if some column leaves [0, stride), a
-          // secondary entry in the phase with the row parity flipped.
-          const bool rows_hit = Yb + 2 * (nY - 1) >= 0 && Yb < g.height;
-          const bool cols_hit = Xb + 2 * (nX - 1) >= 0 && Xb < g.stride;
-          if (rows_hit && cols_hit) {
-            const int c = Xb >> 1, r = Yb >> 1;   // arithmetic shifts: floor for negative coordinates
-            const int band = std::min(std::max(floor_div(r, B), 0), nbands - 1);
-            const int rr = r - band * B;
-            if (rr > -32768 && rr < 32767) {
-              egrp[((size_t)a * nstage + ((Yb & 1) * 2 + (Xb & 1)) * nbands + band) * 4 + (c & 3)].push_back(
-                (int32_t)((uint32_t)(rr & 0xFFFF) | ((uint32_t)(c >> 2) << 16)));
-              ++ne;
-            }
-          }
-          const bool wraps = Xb < 0 || Xb + 2 * (nX - 1) >= g.stride;
-          if (wraps && Yb + 2 * (nY - 1) + 1 >= 0 && Yb - 1 < g.height) {
-            const int r = (Yb - 1) >> 1;
-            const int band = std::min(std::max(floor_div(r, B), 0), nbands - 1);
-            wgrp[(size_t)a * nstage + (((Yb & 1) ^ 1) * 2 + (Xb & 1)) * nbands + band].push_back(
-              (int32_t)((uint32_t)(Xb & 0xFFFF) | ((uint32_t)Yb << 16)));
-          }
-        } else {
-          const int32_t dv = device_offset(off, g.data_size);
-          if (dv != kDevInvalid) slow_a[a].push_back(dv);   // FAR: can still index [0, data_size) for some pose
-        }
-      }
-      nfast_a[a] = nf; nedge_a[a] = ne;
+      classify_beams(g, pl, a, pitch_w, B, nbands, cls[a]);
       // the angle's groups of every stage: table of (plain begin, singles begin, pairs begin, pairs end) per alignment, relative
       // to the angle's own payload (whose start is 4-entry aligned in the block), and the payload
       for (int sg = 0; sg < nstage; ++sg) {
@@ -1119,7 +1121,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
         std::vector<uint16_t> & pay = E.pay;
         pay.clear();
         for (int m = 0; m < 4; ++m) {
-          std::vector<uint16_t> & gk = grp[((size_t)a * nstage + sg) * 4 + m];
+          std::vector<uint16_t> & gk = cls[a].fast[sg * 4 + m];
           std::sort(gk.begin(), gk.end());
           while (pay.size() & 3) pay.push_back(0);   // the plain list is read with 64-bit loads
           const int pb = (int)pay.size();
@@ -1179,18 +1181,18 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     host_parallel_for(nA, one_angle);
     for (int a = 0; a < nA; ++a) {
       slow_start[(size_t)q * (nA + 1) + a] = (int32_t)slow.size();
-      slow.insert(slow.end(), slow_a[a].begin(), slow_a[a].end());
-      n_fast += nfast_a[a]; n_edge += nedge_a[a];
+      slow.insert(slow.end(), cls[a].far.begin(), cls[a].far.end());
+      n_fast += cls[a].n_fast; n_edge += cls[a].n_edge;
     }
     slow_start[(size_t)q * (nA + 1) + nA] = (int32_t)slow.size();
     for (int a = 0; a < nA; ++a)
       for (int sg = 0; sg < nstage; ++sg) {
         wrap2_start[((size_t)q * nA + a) * nstage + sg] = (int32_t)wrap2.size();
-        const auto & w = wgrp[(size_t)a * nstage + sg];
+        const auto & w = cls[a].wrap2[sg];
         wrap2.insert(wrap2.end(), w.begin(), w.end());
         for (int m = 0; m < 4; ++m) {
           edge_start[(((size_t)q * nA + a) * nstage + sg) * 4 + m] = (int32_t)edge.size();
-          const auto & ev = egrp[((size_t)a * nstage + sg) * 4 + m];
+          const auto & ev = cls[a].edge[sg * 4 + m];
           edge.insert(edge.end(), ev.begin(), ev.end());
         }
       }
@@ -1227,7 +1229,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
               ++na;
             }
             nedge.assign((size_t)na * 4, 0);
-            for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)egrp[((size_t)(a + (g2 >> 2)) * nstage + sg) * 4 + (g2 & 3)].size();
+            for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)cls[a + (g2 >> 2)].edge[sg * 4 + (g2 & 3)].size();
             if (!build_block_items(tbl, nedge, na, xtiles, ytiles, items)) return bail(13);
             if (items.size() > 32767) return bail(10);   // TileSeq.nitems is 16-bit
             int32_t * ts = S.tile_stats;
@@ -1253,7 +1255,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
             e.flags = (first_sub ? kSeqNewStage : 0u) | ((first_sub && sg == 0) ? kSeqNewChunk : 0u);
             if (first_sub)
               for (int aa = ca0; aa < ca0 + cna; ++aa)
-                if (!wgrp[(size_t)aa * nstage + sg].empty()) e.flags |= kSeqHasWrap;
+                if (!cls[aa].wrap2[sg].empty()) e.flags |= kSeqHasWrap;
             blob.resize(blob.size() + bytes, 0);
             if (!items.empty()) std::memcpy(blob.data() + e.off, items.data(), items.size() * 8);
             if (!pay.empty()) std::memcpy(blob.data() + e.off + hdr, pay.data(), pay.size() * 2);
@@ -1273,24 +1275,19 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   edge.push_back(0); wrap2.push_back(0); slow.push_back(0);
   blob.resize(blob.size() + 16, 0);
 
-  auto up = [&](auto & dst, const auto & src) {
-    using TT = typename std::remove_reference<decltype(src)>::type::value_type;
-    dst.reserve(src.size());
-    sweep_stage_h2d(dst.p, src.data(), src.size() * sizeof(TT), st);   // pinned arena: no blocking, the vectors may go away
-  };
-  up(S.d_tile_desc, blob);
-  up(S.d_tile_seq, seq);
-  up(S.d_tile_seq_start, seq_start);
-  up(S.d_tile_edge, edge);
-  up(S.d_tile_edge_start, edge_start);
-  up(S.d_tile_wrap2, wrap2);
-  up(S.d_tile_wrap2_start, wrap2_start);
-  up(S.d_tile_slow, slow);
-  up(S.d_tile_slow_start, slow_start);
+  h2d(S.d_tile_desc, blob.data(), blob.size(), st);
+  h2d(S.d_tile_seq, seq.data(), seq.size(), st);
+  h2d(S.d_tile_seq_start, seq_start.data(), seq_start.size(), st);
+  h2d(S.d_edge, edge.data(), edge.size(), st);
+  h2d(S.d_edge_start, edge_start.data(), edge_start.size(), st);
+  h2d(S.d_wrap2, wrap2.data(), wrap2.size(), st);
+  h2d(S.d_wrap2_start, wrap2_start.data(), wrap2_start.size(), st);
+  h2d(S.d_slow, slow.data(), slow.size(), st);
+  h2d(S.d_slow_start, slow_start.data(), slow_start.size(), st);
   T.desc = S.d_tile_desc.p; T.seq = S.d_tile_seq.p; T.seq_start = S.d_tile_seq_start.p;
-  T.edge = S.d_tile_edge.p; T.edge_start = S.d_tile_edge_start.p;
-  T.wrap2 = S.d_tile_wrap2.p; T.wrap2_start = S.d_tile_wrap2_start.p;
-  T.slow = S.d_tile_slow.p; T.slow_start = S.d_tile_slow_start.p;
+  T.edge = S.d_edge.p; T.edge_start = S.d_edge_start.p;
+  T.wrap2 = S.d_wrap2.p; T.wrap2_start = S.d_wrap2_start.p;
+  T.slow = S.d_slow.p; T.slow_start = S.d_slow_start.p;
   T.enabled = 1;
   S.tile_smem = smem;
 
@@ -1316,13 +1313,12 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   S.tile_info[0] = 1; S.tile_info[1] = C; S.tile_info[2] = V; S.tile_info[3] = nbands; S.tile_info[4] = B; S.tile_info[5] = 0;
   S.tile_info[6] = clusters; S.tile_info[7] = (int32_t)(smem / 1024);
   S.tile_layout[0] = ytile_rows; S.tile_layout[1] = ytiles; S.tile_layout[2] = xtiles; S.tile_layout[3] = tail ? 1 : 0;
-  S.fast_info[1] = n_fast; S.fast_info[2] = n_edge; S.fast_info[3] = (int32_t)slow.size() - 1;
+  S.beam_counts[0] = n_fast; S.beam_counts[1] = n_edge; S.beam_counts[2] = (int32_t)slow.size() - 1;
   return true;
 }
 
-void launch_sweep_tile(b200sm * h, SweepHost & S, cudaStream_t st)
+void launch_sweep_tile(SweepHost & S, cudaStream_t st)
 {
-  (void)h;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)S.tile_grid);
   cfg.blockDim = dim3(kTileThreads);

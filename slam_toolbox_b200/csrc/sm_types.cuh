@@ -1,5 +1,5 @@
 // Data structures of the scan matcher shared between scan_matcher.cu (single-match path, C ABI)
-// and sm_sweep.cu (batched loop-closure sweep).
+// and the batched loop-closure sweep (sm_sweep.cu, sm_fast.cu, sm_tile.cu).
 #pragma once
 #include <cstdint>
 #include <functional>
@@ -115,7 +115,7 @@ struct SweepDev {
   PairOut * out;
 };
 
-// Fast sweep path (k_sweep_fast): per-query beam lists in "parity sub-grid" form.
+// Fast sweep path (k_sweep_fast, sm_fast.cu): per-query beam lists in "parity sub-grid" form.
 //   The coarse search steps 2 cells in x and y, so one beam only ever reads grid cells of ONE
 //   (column parity, row parity) class: the grid is kept in shared memory as one parity sub-grid
 //   at a time (4 phases), in which consecutive x-poses are consecutive BYTES -> one 32-bit shared
@@ -195,6 +195,14 @@ struct FineDev {
   int32_t * sums;            // [npairs][P*nA]
 };
 
+// the all-poses-tie result (mean, covariance) of each query, evaluated on first use (finish_query_pair)
+struct ZeroCache {
+  std::vector<char> done;
+  std::vector<double> mean, cov;   // [nq][3], [nq][9]
+};
+
+enum { kSweepGeneric = 0, kSweepFast = 1, kSweepTile = 2 };   // b200sm_batch_info's kernel codes
+
 // host state of an uploaded sweep
 struct SweepHost {
   bool uploaded = false, ran = false;
@@ -209,10 +217,21 @@ struct SweepHost {
     d_cells, d_cell_count, d_ws_sums, d_fine_off, d_fine_pos, d_fine_sums;
   DevBuf<double> d_qgeom, d_center, d_qd, d_angpen, d_points, d_ws_probs;
   DevBuf<uint8_t> d_ws_grid, d_kernel, d_win_flag;
+  // the sweep kernel the upload chose (kSweepGeneric / kSweepFast / kSweepTile) and, when that is the generic kernel, why the
+  // parity kernels were refused (b200sm_batch_info)
+  int kernel = kSweepGeneric;
+  int32_t refused_reason = 0;
+  // EDGE / wrap2 / FAR beam lists of the parity kernel that runs (an upload builds one kernel's tables only)
+  DevBuf<int32_t> d_edge, d_edge_start, d_wrap2, d_wrap2_start, d_slow, d_slow_start;
+  // beam counts of the parity kernel that runs: FAST entries (descriptors of the single-CTA kernel, beams of the tiled one),
+  // EDGE beams, FAR beams
+  int32_t beam_counts[3] = {0, 0, 0};
   DevBuf<uint16_t> d_fast_beams, d_fast_mult;
-  DevBuf<int32_t> d_fast_cls, d_fast_slow, d_fast_slow_start, d_fast_wrap2, d_fast_wrap2_start, d_fast_edge, d_fast_edge_start;
+  DevBuf<int32_t> d_fast_cls;
   FastDev fast{};
   size_t fast_smem = 0;
+  int fast_blocks = 0;
+  int32_t fast_refusal = 0;   // why build_fast_tables last refused a sweep (0 = it built its tables)
   TileDev tile{};
   size_t tile_smem = 0;
   int tile_grid = 0;
@@ -223,9 +242,7 @@ struct SweepHost {
   int32_t tile_layout[4] = {0, 0, 0, 0};   // rows per y-tile (40 or 48), y-tiles, x-tiles, tail row (b200sm_batch_tile_layout)
   DevBuf<uint8_t> d_tile_desc;
   DevBuf<TileSeq> d_tile_seq;
-  DevBuf<int32_t> d_tile_seq_start, d_tile_edge, d_tile_edge_start, d_tile_wrap2, d_tile_wrap2_start, d_tile_slow, d_tile_slow_start;
-  int32_t fast_info[5] = {0, 0, 0, 0, 0};   // enabled, FAST descriptors, CLIP beams, WRAP beams, reason the fast path was refused
-  int fast_blocks = 0;
+  DevBuf<int32_t> d_tile_seq_start;
   DevBuf<PairOut> d_out;
   PinBuf<PairOut> h_out;
   PinBuf<uint8_t> arena;    // pinned staging of the upload's tables (sweep_stage_h2d)
@@ -238,8 +255,7 @@ struct SweepHost {
   // pairs of the last fetch finished by the all-poses-tie closed form / handed to the single-match path
   int zero_pairs = 0, fallback_pairs = 0;
   double upload_ms[3] = {0, 0, 0};   // host wall time of the last upload: lookup tables (plans), kernel tables, whole call
-  std::vector<char> zero_done, zero_exp_done;
-  std::vector<double> zero_mean, zero_cov, zero_exp_mean, zero_exp_cov;   // ... and of the widest response-expansion pass
+  ZeroCache zero, zero_exp;   // all-poses-tie results per query: of the coarse pass, of the widest response-expansion pass
   void release();
 };
 
@@ -289,10 +305,41 @@ double normalize_angle_difference(double minuend, double subtrahend);
 }  // namespace b200
 
 namespace b200 {
-// ScanMatcher::CorrelateScan's reduction + covariance (M.cpp:775-1025) on the host from an integer volume
+// The beams of one query plan and one angle, sorted into the classes of the parity-sub-grid kernels.  A beam's base cell is
+// (Xb, Yb) = (xs[0], ys[0]) + its grid-cell offset; its window covers columns Xb .. Xb + 2 (nX - 1) and rows Yb .. Yb + 2 (nY - 1).
+//   FAST: the window is inside the grid.  A 16-bit word offset into its band of the parity sub-grid, per (stage, alignment m =
+//         sub-column & 3); stage = phase * nbands + band, phase = row parity * 2 + column parity.
+//   EDGE: the window leaves the grid by less than one stride in x, so the reference's linear index (M.cpp:1192-1200) wraps at
+//         most one row.  A primary entry (band-relative sub-row | word << 16) per (stage, m) when some pose reads inside the
+//         grid, and a wrap2 entry (Xb | Yb << 16) per stage of the flipped row parity when some column leaves [0, stride).
+//   FAR:  the other beams that can still index [0, data_size) for some pose: device-form linear offsets.
+struct BeamClasses {
+  std::vector<std::vector<uint16_t>> fast;   // [stage * 4 + m]
+  std::vector<std::vector<int32_t>> edge;    // [stage * 4 + m]
+  std::vector<std::vector<int32_t>> wrap2;   // [stage]
+  std::vector<int32_t> far;
+  int n_fast = 0, n_edge = 0;                // FAST beams, EDGE beams with a primary entry
+};
+// pitch_w = sub-grid row pitch in words; nbands bands of band_rows sub-rows each, the last one open-ended
+void classify_beams(const GridGeom & g, const CorrPlan & pl, int a, int pitch_w, int band_rows, int nbands, BeamClasses & c);
+
+// The builders of the parity kernels' tables return false, with a refusal code in fast_refusal / tile_info[5], when their kernel
+// cannot run the uploaded sweep.  They copy nothing to the device before their last refusal.
+bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st);
 bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st);
+void launch_sweep_fast(SweepHost & S, cudaStream_t st);
+void launch_sweep_tile(SweepHost & S, cudaStream_t st);
+
 void sweep_stage_h2d(void * dst, const void * src, size_t bytes, cudaStream_t s);
-void launch_sweep_tile(b200sm * h, SweepHost & S, cudaStream_t st);
+// count elements into dst (grown as needed) through the upload's pinned staging arena (sweep_stage_h2d)
+template <class T>
+inline void h2d(DevBuf<T> & dst, const T * src, size_t count, cudaStream_t s)
+{
+  dst.reserve(count);
+  sweep_stage_h2d(dst.p, src, count * sizeof(T), s);
+}
+
+// ScanMatcher::CorrelateScan's reduction + covariance (M.cpp:775-1025) on the host from an integer volume
 double host_epilogue(const b200sm_params & prm, const GridGeom & geom, int probs_side, const CorrPlan & pl,
                      const int32_t * sums, bool do_penalize, double mean[3], double cov[9],
                      const std::function<bool(int, int, int32_t *)> * extra_cell = nullptr);

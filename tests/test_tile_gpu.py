@@ -185,3 +185,51 @@ def test_other_search_windows_and_angle_resolutions():
             info = gm.batch_info()
             assert info["kernel"] == "tile", (grid, info)
             assert np.array_equal(r, er) and np.array_equal(m, em) and np.array_equal(c, ec), (grid, cluster, gm.batch_tile_info())
+
+
+def test_plan_readouts_describe_the_last_upload():
+    """One handle, four uploads: tiled kernel, forced generic kernel, single-CTA kernel, tiled kernel again.  The readouts of the
+    kernel choice (batch_info, batch_tile_info, batch_tile_stats) describe the last upload only: the forced generic kernel refused
+    nothing and classified no beams, the single-CTA upload has no tiled plan, and the second tiled upload reads like the first.
+    Every upload runs on its own kernel to the same results.  An order-dependent raster refuses both parity kernels: the generic
+    kernel runs with reason 100 + the tiled planner's refusal code 1."""
+    nq, nch = 2, 6
+    sw = synth.make_loop_sweep(91, n_queries=nq, n_chains=nch, chain_len=2, inf_frac=0.02)
+    mapper = dict(H.MAPPER_LOOP, use_response_expansion=0)
+    gm = H.gpu_matcher(mapper, H.GRID_LOOP)
+    gc, gq = H.gpu_block(sw.cand_ranges, sw.cand_poses), H.gpu_block(sw.query_ranges, sw.query_poses)
+
+    def upload(**opts):
+        for k, v in opts.items():
+            gm.set_option(k, v)
+        gm.batch_upload(gq, gc, sw.chain_start, None, False)
+        gm.batch_run()
+        return (gm.batch_info(), gm.batch_tile_info(), gm.batch_tile_stats()), gm.batch_fetch()
+
+    tile, out = upload(force_generic_sweep=0, sweep_kernel=2)
+    info, plan, stats = tile
+    assert info["kernel"] == "tile" and plan["available"] and stats["blocks"] > 0 and info["fast_descriptors"] > 0, tile
+    results = [out]
+
+    (info, plan, stats), out = upload(force_generic_sweep=1)
+    assert info["kernel"] == "generic" and info["refused_reason"] == 0, info
+    assert info["fast_descriptors"] == info["edge_beams"] == info["far_beams"] == 0, info
+    assert not any(plan.values()) and not any(stats.values()), (plan, stats)
+    results.append(out)
+
+    (info, plan, stats), out = upload(force_generic_sweep=0, sweep_kernel=1)
+    assert info["kernel"] == "fast" and info["refused_reason"] == 0 and info["fast_descriptors"] > 0, info
+    assert not any(plan.values()) and not any(stats.values()), (plan, stats)
+    results.append(out)
+
+    again, out = upload(sweep_kernel=2)
+    assert again == tile, (again, tile)
+    results.append(out)
+    for r in results[1:]:
+        assert all(np.array_equal(a, b) for a, b in zip(r, results[0]))
+
+    seq = synth.make_loop_sweep(92, n_queries=1, n_chains=2, chain_len=1)
+    gs = H.gpu_matcher(H.MAPPER_SEQ, H.GRID_SEQ_YAML)
+    gs.batch_upload(H.gpu_block(seq.query_ranges, seq.query_poses), H.gpu_block(seq.cand_ranges, seq.cand_poses), seq.chain_start)
+    info, plan = gs.batch_info(), gs.batch_tile_info()
+    assert info["kernel"] == "generic" and info["refused_reason"] == 101 and plan["refused_reason"] == 1, (info, plan)
