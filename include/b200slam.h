@@ -377,6 +377,28 @@ int64_t b200og_launch_count(const b200og * h);
 int b200og_create_from_scans(const b200og_params * params, const b200_scan * scans, int32_t n, b200og_info * info,
                              b200og ** out);
 
+/* Map merge (slam_toolbox's merge_maps_kinematic, src/merge_maps_kinematic.cpp): the submaps' scans stay in the store and are
+ * corrected in place.
+ *
+ * transform_scans = MergeMapsKinematic::transformScan (:195-248) on scans [first, first + count), one correction given as
+ * tf2 holds it (basis row-major 3x3, origin x, y, z).  Every unfiltered point p and the sensor position become
+ * ((b[r][0]*x + b[r][1]*y) + b[r][2]*0) + o[r] for r = 0, 1 (tf2::Transform applied to (x, y, 0), unfused), and each
+ * scan's stored bounding box becomes the box of its four corrected corners (min, max, (max x, min y), (min x, max y)).
+ * Corrections compound: a second call transforms the already transformed scans, as the tool's repeated merges do.
+ * sensor_poses = count x 3 host-computed sensor poses for lasers with a mounting offset (only x, y are kept); NULL = the
+ * formula above (exact for a laser at the robot origin).  B200_ERR_INVALID_ARG for a range outside the store or a
+ * non-finite basis / origin.  After the first transform, every build sizes its grid from the union of the stored boxes
+ * (ComputeDimensions reads them: the tool clears IsDirty); before it, a build computes the box from the points as always. */
+int b200og_transform_scans(b200og * h, int32_t first, int32_t count, const double basis[9], const double origin[3],
+                           const double * sensor_poses);
+/* b200og_build over scans [first, first + count) only (one submap's own grid from the shared store); the same results
+ * contract.  B200_ERR_NOT_FOUND for count == 0, B200_ERR_INVALID_ARG for a range outside the store. */
+int b200og_build_range(b200og * h, int32_t first, int32_t count, b200og_info * info);
+/* Per-scan bounding boxes of scans [first, first + count), boxes = count x {min x, min y, max x, max y}: LocalizedRangeScan::
+ * Update's box (sensor position + points whose range is within [minimum_range, range_threshold]) until a transform
+ * replaced it.  b200og_clear_scans drops the boxes and the transformed state. */
+int b200og_scan_boxes(b200og * h, int32_t first, int32_t count, double * boxes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -158,6 +158,9 @@ def lib():
     L.b200og_launch_count.argtypes = [C.c_void_p]
     L.b200og_create_from_scans.argtypes = [C.POINTER(OgParams), C.POINTER(CScan), C.c_int32, C.POINTER(OgInfo),
                                            C.POINTER(C.c_void_p)]
+    L.b200og_transform_scans.argtypes = [C.c_void_p, C.c_int32, C.c_int32, _DP, _DP, _DP]
+    L.b200og_build_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(OgInfo)]
+    L.b200og_scan_boxes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, _DP]
     _lib = L
     return L
 
@@ -623,9 +626,31 @@ class OccupancyGrid:
     def NumScans(self) -> int:
         return lib().b200og_num_scans(self._h)
 
-    def Build(self):
-        _check(lib().b200og_build(self._h, C.byref(self.info)))
+    def Build(self, first: int = 0, count: int | None = None):
+        """CreateFromScans over all stored scans, or over scans [first, first + count) (one submap of a shared store)"""
+        if first == 0 and count is None:
+            _check(lib().b200og_build(self._h, C.byref(self.info)))
+        else:
+            count = self.NumScans() - first if count is None else count
+            _check(lib().b200og_build_range(self._h, int(first), int(count), C.byref(self.info)))
         return self
+
+    def TransformScans(self, first: int, count: int, basis, origin, sensor_poses=None):
+        """slam_toolbox's MergeMapsKinematic::transformScan (src/merge_maps_kinematic.cpp:195-248) in place on scans
+        [first, first + count), with the correction as tf2 holds it: basis (3, 3) and origin (3,).  Points, sensor positions
+        and stored boxes are corrected on the device; corrections compound across calls.  sensor_poses = (count, 3) poses
+        computed on the host for a laser with a mounting offset (None: the sensor position takes the points' formula)."""
+        b = np.ascontiguousarray(basis, dtype=np.float64).reshape(9)
+        o = np.ascontiguousarray(origin, dtype=np.float64).reshape(3)
+        sp = None if sensor_poses is None else np.ascontiguousarray(sensor_poses, dtype=np.float64).reshape(int(count), 3)
+        _check(lib().b200og_transform_scans(self._h, int(first), int(count), _dp(b), _dp(o), None if sp is None else _dp(sp)))
+
+    def ScanBoxes(self, first: int = 0, count: int | None = None) -> np.ndarray:
+        """(count, 4) per-scan bounding boxes {min x, min y, max x, max y} as the store holds them"""
+        count = self.NumScans() - first if count is None else count
+        out = np.zeros((max(int(count), 0), 4))
+        _check(lib().b200og_scan_boxes(self._h, int(first), int(count), _dp(out)))
+        return out
 
     def GetWidth(self) -> int:
         return self.info.width

@@ -15,6 +15,15 @@
 //                into one RED.ADD of the run length (no return value) -- integer sums commute, so the
 //                result does not depend on the order and equals the reference's sequential loop
 //   k_og_update  counters -> cell state (UpdateCell Karto.h:6241-6254), FP64 ratio test as the reference
+// A build over a scan range [first, first + count) (b200og_build_range) runs the same kernels through the beam prefix.
+//
+// Map merge (slam_toolbox's merge_maps_kinematic, src/merge_maps_kinematic.cpp:195-310), on the resident store:
+//   box [S][4]   per-scan bounding box {min x, min y, max x, max y}; filled lazily (k_og_scan_box, LocalizedRangeScan::
+//                Update's box) on the first transform or box read-back, so add_scans and a plain build cost what they did
+//   k_og_transform  one rigid correction (tf2 basis / origin) applied in place to the points, sensor positions and boxes
+//                of a scan range, as transformScan does (:195-248); corrections compound across calls like the tool's
+//   k_og_box_union  once any scan was transformed the stored boxes are authoritative (the tool clears IsDirty, so
+//                ComputeDimensions reads them, Karto.h:6088-6112) and a build sizes the grid from their union
 // Beam groups of DIFFERENT scans are interleaved over the warps so that the cells next to one sensor
 // (which every beam of that scan crosses) are not hammered by the whole grid at the same time.
 //
@@ -28,6 +37,7 @@
 #include <memory>
 #include <mutex>
 #include <stdexcept>
+#include <string>
 #include <vector>
 
 #include "common.cuh"
@@ -45,7 +55,7 @@ struct OgDev {
   const double * sensor;
   const int32_t * start;
   int32_t nscans, maxbeams;
-  int64_t nbeams;
+  int64_t beam0, nbeams;   // beams [beam0, nbeams) of the built scan range (absolute store indices)
   double rt, minr, maxr;
   double scale, offx, offy;
   int32_t width, height, stride;
@@ -73,7 +83,7 @@ __global__ void __launch_bounds__(kOgThreads) k_og_bbox(OgDev d, double * partia
   const double big = 999999999999999999.99999;
   double mnx = big, mny = big, mxx = -big, mxy = -big;
   const int64_t step = (int64_t)gridDim.x * blockDim.x, t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  for (int64_t i = t0; i < d.nbeams; i += step) {
+  for (int64_t i = d.beam0 + t0; i < d.nbeams; i += step) {
     const double r = d.ranges[i];
     if (r >= d.minr && r <= d.rt) {   // math::InRange (Math.h:123), LocalizedRangeScan::Update Karto.h:5662
       const double x = d.points[2 * i], y = d.points[2 * i + 1];
@@ -89,6 +99,120 @@ __global__ void __launch_bounds__(kOgThreads) k_og_bbox(OgDev d, double * partia
     if (y < mny) mny = y;
     if (x > mxx) mxx = x;
     if (y > mxy) mxy = y;
+  }
+  mnx = warp_min(mnx); mny = warp_min(mny); mxx = warp_max(mxx); mxy = warp_max(mxy);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) { sm[0][w] = mnx; sm[1][w] = mny; sm[2][w] = mxx; sm[3][w] = mxy; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < kOgThreads / 32; ++k) {
+      if (sm[0][k] < mnx) mnx = sm[0][k];
+      if (sm[1][k] < mny) mny = sm[1][k];
+      if (sm[2][k] > mxx) mxx = sm[2][k];
+      if (sm[3][k] > mxy) mxy = sm[3][k];
+    }
+    double * o = partial + 4 * (size_t)blockIdx.x;
+    o[0] = mnx; o[1] = mny; o[2] = mxx; o[3] = mxy;
+  }
+}
+
+// LocalizedRangeScan::Update's box of every scan in [first, first + count) (Karto.h:5662-5698): one warp per scan, the
+// in-range points and the sensor position, from BoundingBox2's +-999999999999999999.99999.  box[s] = {min x, min y, max x, max y}
+__global__ void __launch_bounds__(kOgThreads) k_og_scan_box(OgDev d, int32_t first, int32_t count, double * box)
+{
+  const double big = 999999999999999999.99999;
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * (kOgThreads / 32);
+  for (int64_t k = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); k < count; k += nwarps) {
+    const int32_t s = first + (int32_t)k;
+    double mnx = big, mny = big, mxx = -big, mxy = -big;
+    for (int64_t i = d.start[s] + lane; i < d.start[s + 1]; i += 32) {
+      const double r = d.ranges[i];
+      if (r >= d.minr && r <= d.rt) {
+        const double x = d.points[2 * i], y = d.points[2 * i + 1];
+        if (x < mnx) mnx = x;
+        if (y < mny) mny = y;
+        if (x > mxx) mxx = x;
+        if (y > mxy) mxy = y;
+      }
+    }
+    mnx = warp_min(mnx); mny = warp_min(mny); mxx = warp_max(mxx); mxy = warp_max(mxy);
+    if (lane == 0) {
+      const double x = d.sensor[2 * s], y = d.sensor[2 * s + 1];
+      if (x < mnx) mnx = x;
+      if (y < mny) mny = y;
+      if (x > mxx) mxx = x;
+      if (y > mxy) mxy = y;
+      double * o = box + 4 * (size_t)s;
+      o[0] = mnx; o[1] = mny; o[2] = mxx; o[3] = mxy;
+    }
+  }
+}
+
+// One correction as tf2 holds it: rows 0 and 1 of basis[3][3], origin x, y.
+struct OgTf {
+  double b[2][3];
+  double o[2];
+};
+
+// tf2::Transform::operator()(Vector3(x, y, 0)): the basis row dot product, then + origin, in this order and unfused
+// (the unit is compiled with -fmad=false) -- MergeMapsKinematic::applyCorrection, src/merge_maps_kinematic.cpp:180-192
+__device__ __forceinline__ void og_apply(const OgTf & t, double x, double y, double & ox, double & oy)
+{
+  ox = ((t.b[0][0] * x + t.b[0][1] * y) + t.b[0][2] * 0.0) + t.o[0];
+  oy = ((t.b[1][0] * x + t.b[1][1] * y) + t.b[1][2] * 0.0) + t.o[1];
+}
+
+// transformScan (src/merge_maps_kinematic.cpp:195-248) on scans [first, first + count): every unfiltered point, the sensor
+// position (when the host did not supply it) and the stored box, replaced by the box of its four corrected corners added
+// in the tool's order: min, max, (max x, min y), (min x, max y) (:206-221).  Ranges are untouched.
+__global__ void __launch_bounds__(kOgThreads) k_og_transform(OgDev d, int32_t first, int32_t count, OgTf t, int32_t do_sensor,
+                                                             double * points, double * sensor, double * box)
+{
+  const int64_t step = (int64_t)gridDim.x * blockDim.x, t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  for (int64_t i = d.beam0 + t0; i < d.nbeams; i += step) {
+    double x, y;
+    og_apply(t, points[2 * i], points[2 * i + 1], x, y);
+    points[2 * i] = x; points[2 * i + 1] = y;
+  }
+  const double big = 999999999999999999.99999;
+  for (int64_t k = t0; k < count; k += step) {
+    const int64_t s = first + k;
+    if (do_sensor) {
+      double x, y;
+      og_apply(t, sensor[2 * s], sensor[2 * s + 1], x, y);
+      sensor[2 * s] = x; sensor[2 * s + 1] = y;
+    }
+    double * bx = box + 4 * s;
+    const double cx[4] = {bx[0], bx[2], bx[2], bx[0]}, cy[4] = {bx[1], bx[3], bx[1], bx[3]};
+    double mnx = big, mny = big, mxx = -big, mxy = -big;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {   // BoundingBox2::Add, Karto.h:2897-2901
+      double x, y;
+      og_apply(t, cx[c], cy[c], x, y);
+      if (x < mnx) mnx = x;
+      if (y < mny) mny = y;
+      if (x > mxx) mxx = x;
+      if (y > mxy) mxy = y;
+    }
+    bx[0] = mnx; bx[1] = mny; bx[2] = mxx; bx[3] = mxy;
+  }
+}
+
+// ComputeDimensions over stored boxes (Karto.h:6097-6104, BoundingBox2::Add(BoundingBox2) :2906-2910): partial[block][4] like
+// k_og_bbox, the union of box[first .. first + count)
+__global__ void __launch_bounds__(kOgThreads) k_og_box_union(const double * box, int32_t first, int32_t count, double * partial)
+{
+  __shared__ double sm[4][kOgThreads / 32];
+  const double big = 999999999999999999.99999;
+  double mnx = big, mny = big, mxx = -big, mxy = -big;
+  const int64_t step = (int64_t)gridDim.x * blockDim.x, t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  for (int64_t k = t0; k < count; k += step) {
+    const double * b = box + 4 * (first + k);
+    if (b[0] < mnx) mnx = b[0];
+    if (b[1] < mny) mny = b[1];
+    if (b[2] > mxx) mxx = b[2];
+    if (b[3] > mxy) mxy = b[3];
   }
   mnx = warp_min(mnx); mny = warp_min(mny); mxx = warp_max(mxx); mxy = warp_max(mxy);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
@@ -255,6 +379,10 @@ struct b200og {
   GrowBuf<int32_t> d_start;
   std::vector<int32_t> start{0};
   int32_t maxbeams = 0;
+  // merge state: per-scan boxes of scans [0, nboxed), authoritative once a transform ran (boxes_auth)
+  GrowBuf<double> d_box;
+  int32_t nboxed = 0;
+  bool boxes_auth = false;
   // staging (two pinned halves, filled while the other one is in flight)
   double * stage[2] = {nullptr, nullptr};
   cudaEvent_t stage_done[2] = {nullptr, nullptr};
@@ -411,27 +539,120 @@ int add_scans(b200og * h, const b200_scan * scans, int32_t n)
   return B200_OK;
 }
 
-int build(b200og * h, b200og_info * info)
+// the store's view of scans [first, first + count): start / sensor shifted to the first scan, beams through the prefix
+OgDev range_view(const b200og * h, int32_t first, int32_t count)
+{
+  OgDev d{};
+  d.ranges = h->d_ranges.p; d.points = h->d_points.p; d.sensor = h->d_sensor.p + 2 * (size_t)first; d.start = h->d_start.p + first;
+  d.nscans = count;
+  d.beam0 = h->start[first]; d.nbeams = h->start[first + count];
+  if (first == 0 && count == h->nscans()) {
+    d.maxbeams = h->maxbeams;
+  } else {
+    for (int32_t s = first; s < first + count; ++s) d.maxbeams = std::max(d.maxbeams, h->start[s + 1] - h->start[s]);
+  }
+  d.rt = h->p.range_threshold; d.minr = h->p.minimum_range; d.maxr = h->p.maximum_range;
+  return d;
+}
+
+bool range_ok(const b200og * h, int32_t first, int32_t count, const char * who)
+{
+  if (first < 0 || count < 0 || (int64_t)first + count > h->nscans()) {
+    set_last_error(std::string(who) + ": scan range outside the store");
+    return false;
+  }
+  return true;
+}
+
+// Update's box for every scan that has none yet (scans appended since the last call included)
+void ensure_boxes(b200og * h)
+{
+  const int32_t n = h->nscans();
+  if (h->nboxed == n) return;
+  h->ensure_stream();
+  h->d_box.ensure(4 * (size_t)n, 4 * (size_t)h->nboxed, h->stream);
+  const OgDev d = range_view(h, 0, n);
+  const int32_t count = n - h->nboxed;
+  const int nb = (int)std::min<int64_t>(((int64_t)count + kOgThreads / 32 - 1) / (kOgThreads / 32), (int64_t)h->sms * 8);
+  k_og_scan_box<<<std::max(nb, 1), kOgThreads, 0, h->stream>>>(d, h->nboxed, count, h->d_box.p);
+  B200_CUDA(cudaGetLastError());
+  ++h->launches;
+  h->nboxed = n;
+}
+
+int transform_scans(b200og * h, int32_t first, int32_t count, const double * basis, const double * origin, const double * sensor_poses)
+{
+  if (!basis || !origin) { set_last_error("b200og_transform_scans: NULL basis or origin"); return B200_ERR_INVALID_ARG; }
+  if (!range_ok(h, first, count, "b200og_transform_scans")) return B200_ERR_INVALID_ARG;
+  for (int k = 0; k < 9; ++k)
+    if (!std::isfinite(basis[k])) { set_last_error("b200og_transform_scans: non-finite basis"); return B200_ERR_INVALID_ARG; }
+  for (int k = 0; k < 3; ++k)
+    if (!std::isfinite(origin[k])) { set_last_error("b200og_transform_scans: non-finite origin"); return B200_ERR_INVALID_ARG; }
+  if (count == 0) return B200_OK;
+  ensure_boxes(h);
+  cudaStream_t st = h->stream;
+  if (sensor_poses) {   // host-computed sensor poses (lasers with a mounting offset): positions only
+    std::vector<double> xy(2 * (size_t)count);
+    for (int32_t s = 0; s < count; ++s) { xy[2 * s] = sensor_poses[3 * s]; xy[2 * s + 1] = sensor_poses[3 * s + 1]; }
+    B200_CUDA(cudaMemcpyAsync(h->d_sensor.p + 2 * (size_t)first, xy.data(), xy.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  }
+  OgTf t;
+  for (int r = 0; r < 2; ++r) {
+    for (int c = 0; c < 3; ++c) t.b[r][c] = basis[3 * r + c];
+    t.o[r] = origin[r];
+  }
+  const OgDev d = range_view(h, first, count);
+  const int64_t work = std::max<int64_t>(d.nbeams - d.beam0, count);
+  const int nb = (int)std::min<int64_t>((work + kOgThreads - 1) / kOgThreads, (int64_t)h->sms * 8);
+  B200_CUDA(cudaEventRecord(h->ev0, st));
+  k_og_transform<<<std::max(nb, 1), kOgThreads, 0, st>>>(d, first, count, t, sensor_poses ? 0 : 1, h->d_points.p, h->d_sensor.p,
+                                                         h->d_box.p);
+  B200_CUDA(cudaGetLastError());
+  ++h->launches;
+  B200_CUDA(cudaEventRecord(h->ev1, st));
+  B200_CUDA(cudaStreamSynchronize(st));   // the host staging of sensor_poses is released on return
+  B200_CUDA(cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+  h->boxes_auth = true;
+  h->built = false;
+  return B200_OK;
+}
+
+int scan_boxes(b200og * h, int32_t first, int32_t count, double * boxes)
+{
+  if (!range_ok(h, first, count, "b200og_scan_boxes") || (count > 0 && !boxes)) {
+    if (count > 0 && !boxes) set_last_error("b200og_scan_boxes: NULL output");
+    return B200_ERR_INVALID_ARG;
+  }
+  if (count == 0) return B200_OK;
+  ensure_boxes(h);
+  B200_CUDA(cudaMemcpyAsync(boxes, h->d_box.p + 4 * (size_t)first, 4 * (size_t)count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200_OK;
+}
+
+int build(b200og * h, int32_t first, int32_t count, b200og_info * info)
 {
   if (info) std::memset(info, 0, sizeof(*info));
   h->built = false;
-  if (h->nscans() == 0) {
+  if (count == 0) {
     set_last_error("OccupancyGrid::CreateFromScans: no scans (the reference returns NULL, Karto.h:5950-5952)");
     return B200_ERR_NOT_FOUND;
   }
   h->ensure_stream();
   cudaStream_t st = h->stream;
-  OgDev d{};
-  d.ranges = h->d_ranges.p; d.points = h->d_points.p; d.sensor = h->d_sensor.p; d.start = h->d_start.p;
-  d.nscans = h->nscans(); d.maxbeams = h->maxbeams; d.nbeams = h->start.back();
-  d.rt = h->p.range_threshold; d.minr = h->p.minimum_range; d.maxr = h->p.maximum_range;
+  OgDev d = range_view(h, first, count);
   const int blocks = h->sms * 8;
   h->d_partial.reserve(4 * (size_t)blocks);
   h->h_partial.reserve(4 * (size_t)blocks);
   h->d_flag.reserve(1);
   h->h_flag.reserve(1);
   B200_CUDA(cudaEventRecord(h->ev0, st));
-  k_og_bbox<<<blocks, kOgThreads, 0, st>>>(d, h->d_partial.p);
+  if (h->boxes_auth) {   // transformed store: the union of the stored boxes (ComputeDimensions reads them, IsDirty is clear)
+    ensure_boxes(h);
+    k_og_box_union<<<blocks, kOgThreads, 0, st>>>(h->d_box.p, first, count, h->d_partial.p);
+  } else {
+    k_og_bbox<<<blocks, kOgThreads, 0, st>>>(d, h->d_partial.p);
+  }
   B200_CUDA(cudaGetLastError());
   ++h->launches;
   B200_CUDA(cudaMemcpyAsync(h->h_partial.p, h->d_partial.p, 4 * (size_t)blocks * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -557,6 +778,8 @@ int b200og_clear_scans(b200og * h)
   if (!h) return B200_ERR_INVALID_ARG;
   h->start.assign(1, 0);
   h->maxbeams = 0;
+  h->nboxed = 0;
+  h->boxes_auth = false;
   h->built = false;
   return B200_OK;
 }
@@ -567,7 +790,34 @@ int b200og_build(b200og * h, b200og_info * info)
 {
   B200_GUARD_BEGIN
   if (!h) return B200_ERR_INVALID_ARG;
-  return build(h, info);
+  return build(h, 0, h->nscans(), info);
+  B200_GUARD_END
+}
+
+int b200og_build_range(b200og * h, int32_t first, int32_t count, b200og_info * info)
+{
+  B200_GUARD_BEGIN
+  if (info) std::memset(info, 0, sizeof(*info));
+  if (!h) return B200_ERR_INVALID_ARG;
+  if (!range_ok(h, first, count, "b200og_build_range")) return B200_ERR_INVALID_ARG;
+  return build(h, first, count, info);
+  B200_GUARD_END
+}
+
+int b200og_transform_scans(b200og * h, int32_t first, int32_t count, const double basis[9], const double origin[3],
+                           const double * sensor_poses)
+{
+  B200_GUARD_BEGIN
+  if (!h) return B200_ERR_INVALID_ARG;
+  return transform_scans(h, first, count, basis, origin, sensor_poses);
+  B200_GUARD_END
+}
+
+int b200og_scan_boxes(b200og * h, int32_t first, int32_t count, double * boxes)
+{
+  B200_GUARD_BEGIN
+  if (!h) return B200_ERR_INVALID_ARG;
+  return scan_boxes(h, first, count, boxes);
   B200_GUARD_END
 }
 
@@ -626,7 +876,7 @@ int b200og_create_from_scans(const b200og_params * params, const b200_scan * sca
   if (rc != B200_OK) return rc;
   std::unique_ptr<b200og, void (*)(b200og *)> h(raw, b200og_destroy);
   rc = add_scans(h.get(), scans, n);
-  if (rc == B200_OK) rc = build(h.get(), info);
+  if (rc == B200_OK) rc = build(h.get(), 0, h->nscans(), info);
   if (rc != B200_OK) return rc;
   *out = h.release();
   return B200_OK;
