@@ -399,6 +399,16 @@ int b200og_build_range(b200og * h, int32_t first, int32_t count, b200og_info * i
  * replaced it.  b200og_clear_scans drops the boxes and the transformed state. */
 int b200og_scan_boxes(b200og * h, int32_t first, int32_t count, double * boxes);
 
+/* Removes the scans at store indices indices[0 .. n) (strictly increasing) and compacts the store on the device: the
+ * survivors keep their order, and every later call sees exactly the store a fresh handle loaded with the surviving scans
+ * (their transformed values, after a transform) would hold, so builds give bit-identical grids.  Stored boxes and the
+ * transformed state are kept.  Only scans after the first removed one move.  n == 0 does nothing; removing every scan
+ * leaves an empty store.  B200_ERR_INVALID_ARG, with the store unchanged, for a NULL indices with n > 0, n < 0, an index
+ * outside the store, or indices not strictly increasing.  b200og_kernel_ms reads the compaction kernel's time afterwards.
+ * The first removal that moves scans allocates a second copy of the store's device arrays (the compaction target, swapped
+ * with the store after each removal) and keeps it for the handle's life: the store's device footprint doubles. */
+int b200og_remove_scans(b200og * h, const int32_t * indices, int32_t n);
+
 #ifdef __cplusplus
 }
 #endif

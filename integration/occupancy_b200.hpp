@@ -11,6 +11,8 @@
 // bytes, which is everything its consumers read (vis_utils::toNavMap, include/slam_toolbox/
 // visualization_utils.hpp:108-146; map_saver; RayCast / IsFree).  The hit / pass counter grids inside it
 // stay empty: they are scratch of the CPU build (fetch them with b200og_fetch when wanted).
+//
+// ResidentOccupancyMap is the same publish with the scans kept on the device between calls (section 3a).
 #pragma once
 #include <cstdio>
 #include <cstring>
@@ -22,15 +24,16 @@
 namespace karto {
 namespace b200 {
 
-inline OccupancyGrid * CreateOccupancyGridFromScans(const LocalizedRangeScanVector & rScans, kt_double resolution,
-                                                     float * device_ms = nullptr)
+namespace detail {
+
+// the non-NULL scans of rScans as the C ABI takes them (pointers into the scans), and the laser of the first one
+inline std::vector<b200_scan> CollectScans(const LocalizedRangeScanVector & rScans, LaserRangeFinder ** laser)
 {
   std::vector<b200_scan> scans;
-  LaserRangeFinder * laser = nullptr;
   static_assert(sizeof(Vector2<kt_double>) == 2 * sizeof(double), "Vector2<double> must be {x, y}");
   for (LocalizedRangeScan * s : rScans) {
     if (s == nullptr) continue;                                   // Karto.h:6094, :6123
-    if (!laser) laser = s->GetLaserRangeFinder();
+    if (laser && !*laser) *laser = s->GetLaserRangeFinder();
     b200_scan o;
     const PointVectorDouble & pts = s->GetPointReadings(false);  // Karto.h:6149
     o.n = static_cast<int32_t>(pts.size());
@@ -40,7 +43,11 @@ inline OccupancyGrid * CreateOccupancyGridFromScans(const LocalizedRangeScanVect
     o.sensor_pose[0] = p.GetX(); o.sensor_pose[1] = p.GetY(); o.sensor_pose[2] = p.GetHeading();
     scans.push_back(o);
   }
-  if (rScans.empty()) return NULL;                                // Karto.h:5950-5952
+  return scans;
+}
+
+inline b200og_params GridParams(kt_double resolution, LaserRangeFinder * laser)
+{
   b200og_params p;
   b200og_default_params(&p);                                      // MinPassThrough 2, OccupancyThreshold 0.1
   p.resolution = resolution;
@@ -49,22 +56,140 @@ inline OccupancyGrid * CreateOccupancyGridFromScans(const LocalizedRangeScanVect
     p.minimum_range = laser->GetMinimumRange();
     p.maximum_range = laser->GetMaximumRange();
   }
-  b200og * h = nullptr;
-  b200og_info info;
-  if (b200og_create_from_scans(&p, scans.data(), static_cast<int32_t>(scans.size()), &info, &h) != B200_OK) {
-    std::fprintf(stderr, "OccupancyGrid::CreateFromScans (b200): %s\n", b200_last_error());
-    return NULL;
-  }
+  return p;
+}
+
+// the karto grid of a successful build of h
+inline OccupancyGrid * FetchGrid(b200og * h, const b200og_info & info, kt_double resolution)
+{
   OccupancyGrid * g = new OccupancyGrid(info.width, info.height, Vector2<kt_double>(info.offset[0], info.offset[1]), resolution);
   if (g->GetWidthStep() != info.stride || b200og_fetch(h, g->GetDataPointer(), nullptr, nullptr) != B200_OK) {
     std::fprintf(stderr, "OccupancyGrid::CreateFromScans (b200): %s\n", b200_last_error());
     delete g;
     g = NULL;
   }
+  return g;
+}
+
+}  // namespace detail
+
+inline OccupancyGrid * CreateOccupancyGridFromScans(const LocalizedRangeScanVector & rScans, kt_double resolution,
+                                                     float * device_ms = nullptr)
+{
+  LaserRangeFinder * laser = nullptr;
+  const std::vector<b200_scan> scans = detail::CollectScans(rScans, &laser);
+  if (rScans.empty()) return NULL;                                // Karto.h:5950-5952
+  const b200og_params p = detail::GridParams(resolution, laser);
+  b200og * h = nullptr;
+  b200og_info info;
+  if (b200og_create_from_scans(&p, scans.data(), static_cast<int32_t>(scans.size()), &info, &h) != B200_OK) {
+    std::fprintf(stderr, "OccupancyGrid::CreateFromScans (b200): %s\n", b200_last_error());
+    return NULL;
+  }
+  OccupancyGrid * g = detail::FetchGrid(h, info, resolution);
   if (device_ms) b200og_kernel_ms(h, device_ms);
   b200og_destroy(h);
   return g;
 }
+
+// The map publish with the scans resident on the device between publishes.  The store holds the scans of the last publish in
+// the order GetAllProcessedScans returned them (unique-id order).  A publish
+//   - removes, in place (b200og_remove_scans), the stored scans the mapper no longer holds, such as the localization rolling
+//     buffer's oldest scans;
+//   - appends the scans whose unique ids are larger than every stored one (unique ids only grow);
+//   - reloads every scan when poses_corrected is set, i.e. when MapperGraph::CorrectPoses has run since the last publish
+//     (b200_shim_correct_poses_calls() of integration/scan_matcher_b200.cpp counts its calls), since that moves stored scans'
+//     points, and whenever the scans are not in increasing unique-id order.
+// The grid equals CreateOccupancyGridFromScans over the same scans.  One instance per map; not thread-safe.
+class ResidentOccupancyMap {
+ public:
+  struct Stats { int32_t removed = 0, appended = 0, reloaded = 0; };
+
+  ResidentOccupancyMap() = default;
+  ResidentOccupancyMap(const ResidentOccupancyMap &) = delete;
+  ResidentOccupancyMap & operator=(const ResidentOccupancyMap &) = delete;
+  ~ResidentOccupancyMap() { if (h_) b200og_destroy(h_); }
+
+  OccupancyGrid * Publish(const LocalizedRangeScanVector & rScans, kt_double resolution, bool poses_corrected, Stats * stats = nullptr,
+                          float * device_ms = nullptr)
+  {
+    Stats st;
+    std::vector<LocalizedRangeScan *> live;
+    for (LocalizedRangeScan * s : rScans)
+      if (s) live.push_back(s);
+    if (rScans.empty()) { if (stats) *stats = st; return NULL; }  // Karto.h:5950-5952
+    // the grid parameters as CreateOccupancyGridFromScans takes them on every call: the resolution and the first scan's laser
+    // limits.  The store is built for one set; another set starts a fresh store.
+    const b200og_params p = detail::GridParams(resolution, live.empty() ? nullptr : live[0]->GetLaserRangeFinder());
+    if (!h_ || !SameParams(p, params_)) {
+      if (h_) b200og_destroy(h_);
+      h_ = nullptr;
+      ids_.clear();
+      if (b200og_create(&p, &h_) != B200_OK) return Fail();
+      params_ = p;
+      poses_corrected = true;
+    }
+    bool increasing = true;
+    for (size_t k = 1; k < live.size() && increasing; ++k) increasing = live[k - 1]->GetUniqueId() < live[k]->GetUniqueId();
+    // stored scans that are gone, and where the new ones start
+    std::vector<int32_t> gone;
+    size_t next = 0;
+    bool reload = poses_corrected || !increasing;
+    for (size_t k = 0; k < ids_.size() && !reload; ++k) {
+      if (next < live.size() && live[next]->GetUniqueId() == ids_[k]) { ++next; continue; }
+      if (next < live.size() && live[next]->GetUniqueId() < ids_[k]) reload = true;   // a scan older than a stored one is new
+      else gone.push_back(static_cast<int32_t>(k));
+    }
+    if (reload) {
+      if (b200og_clear_scans(h_) != B200_OK) return Fail();
+      ids_.clear();
+      next = 0;
+      st.reloaded = 1;
+    } else if (!gone.empty()) {
+      if (b200og_remove_scans(h_, gone.data(), static_cast<int32_t>(gone.size())) != B200_OK) return Fail();
+      std::vector<kt_int32s> kept;
+      kept.reserve(ids_.size() - gone.size());
+      for (size_t k = 0, r = 0; k < ids_.size(); ++k) {
+        if (r < gone.size() && gone[r] == static_cast<int32_t>(k)) { ++r; continue; }
+        kept.push_back(ids_[k]);
+      }
+      ids_.swap(kept);
+      st.removed = static_cast<int32_t>(gone.size());
+    }
+    const LocalizedRangeScanVector added(live.begin() + next, live.end());
+    const std::vector<b200_scan> scans = detail::CollectScans(added, nullptr);
+    if (!scans.empty() && b200og_add_scans(h_, scans.data(), static_cast<int32_t>(scans.size())) != B200_OK) return Fail();
+    for (LocalizedRangeScan * s : added) ids_.push_back(s->GetUniqueId());
+    st.appended = static_cast<int32_t>(scans.size());
+    if (stats) *stats = st;
+    b200og_info info;
+    if (b200og_build(h_, &info) != B200_OK) return Fail();
+    if (device_ms) b200og_kernel_ms(h_, device_ms);
+    return detail::FetchGrid(h_, info, resolution);
+  }
+
+ private:
+  static bool SameParams(const b200og_params & a, const b200og_params & b)
+  {
+    return a.resolution == b.resolution && a.range_threshold == b.range_threshold && a.minimum_range == b.minimum_range &&
+           a.maximum_range == b.maximum_range && a.min_pass_through == b.min_pass_through &&
+           a.occupancy_threshold == b.occupancy_threshold;
+  }
+
+  // after a failed call the store's contents are unknown: the next publish starts from a fresh handle
+  OccupancyGrid * Fail()
+  {
+    std::fprintf(stderr, "ResidentOccupancyMap (b200): %s\n", b200_last_error());
+    if (h_) b200og_destroy(h_);
+    h_ = nullptr;
+    ids_.clear();
+    return NULL;
+  }
+
+  b200og * h_ = nullptr;
+  b200og_params params_{};       // what h_ was created with
+  std::vector<kt_int32s> ids_;   // unique ids of the stored scans, in store order
+};
 
 }  // namespace b200
 }  // namespace karto

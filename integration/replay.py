@@ -66,6 +66,9 @@ def _bind(which: str):
     L.krep_solver_computes.argtypes = [C.c_void_p, _DP, C.POINTER(C.c_int), C.c_int]
     L.krep_occupancy.restype = C.c_double
     L.krep_occupancy.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(C.c_int), _DP, C.POINTER(C.c_uint8), C.c_long]
+    L.krep_occupancy_resident.restype = C.c_double
+    L.krep_occupancy_resident.argtypes = [C.c_void_p, C.c_double, C.POINTER(C.c_int), _DP, C.POINTER(C.c_uint8), C.c_long,
+                                          C.POINTER(C.c_int), C.POINTER(C.c_float)]
     L.krep_init_laser.argtypes = [C.c_double] * 6
     return L
 
@@ -118,16 +121,38 @@ def _occupancy(L, h, map_resolution: float, out: dict):
         out[f"map_{tag}_cells"] = cells
 
 
+def _publish_pair(L, h, map_resolution: float, step: int, log: list):
+    """One map publish through the resident store (krep_occupancy_resident) and through the reference's CreateFromScans over
+    the same scans.  Appends [step, equal, removed, appended, reloaded, resident seconds, reference seconds, resident device ms]."""
+    info, off, stats, dms = (C.c_int * 3)(), np.zeros(2), (C.c_int * 3)(), C.c_float()
+    cells = np.zeros(1, dtype=np.uint8)
+    sec = L.krep_occupancy_resident(h, map_resolution, info, off.ctypes.data_as(_DP), None, 0, stats, C.byref(dms))
+    if sec >= 0:   # the store is current after the first call: the second one only rebuilds and fetches
+        cells = np.zeros(max(info[1], 0) * max(info[2], 0), dtype=np.uint8)
+        L.krep_occupancy_resident(h, map_resolution, info, off.ctypes.data_as(_DP), cells.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                  cells.size, None, None)
+    rinfo, roff = (C.c_int * 3)(), np.zeros(2)
+    rsec = L.krep_occupancy(h, map_resolution, 0, rinfo, roff.ctypes.data_as(_DP), None, 0)
+    rcells = np.zeros(max(rinfo[1], 0) * max(rinfo[2], 0), dtype=np.uint8)
+    if rsec >= 0:
+        rsec = L.krep_occupancy(h, map_resolution, 0, rinfo, roff.ctypes.data_as(_DP), rcells.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                rcells.size)
+    equal = sec >= 0 and rsec >= 0 and rinfo[:] == info[:] and roff.tobytes() == off.tobytes() and np.array_equal(cells, rcells)
+    log.append([step, int(equal), stats[0], stats[1], stats[2], sec, rsec, dms.value])
+
+
 def run_inprocess(which: str, ranges: np.ndarray, odom: np.ndarray, params: dict, laser: dict, use_solver: bool = True,
-                  map_resolution: float = 0.0):
+                  map_resolution: float = 0.0, publish_every: int = 0):
     L = _bind(which)
     h = _create(L, laser, params, use_solver)
     ranges = np.ascontiguousarray(ranges, dtype=np.float64)
     odom = np.ascontiguousarray(odom, dtype=np.float64)
-    kept = []
+    kept, publishes = [], []
     for i in range(len(ranges)):
         if L.krep_process(h, ranges[i].ctypes.data_as(_DP), ranges.shape[1], odom[i].ctypes.data_as(_DP), i):
             kept.append(i)
+        if publish_every and (i + 1) % publish_every == 0:
+            _publish_pair(L, h, map_resolution, i, publishes)
     _, poses = _scans(L, h)
     n = len(poses)
     st = np.zeros(5)
@@ -141,11 +166,14 @@ def run_inprocess(which: str, ranges: np.ndarray, odom: np.ndarray, params: dict
                process_seconds=st[0], solver_computes=int(st[1]), solver_ms=st[2], edges=int(st[3]), scans=int(st[4]), match_calls=matches)
     if map_resolution:
         _occupancy(L, h, map_resolution, out)
+    if publish_every:
+        out["publishes"] = np.array(publishes, dtype=np.float64).reshape(-1, 8)
     return out
 
 
-def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpdir=None, map_resolution=0.0):
-    """Runs the replay in a fresh process and returns its result dict."""
+def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpdir=None, map_resolution=0.0, publish_every=0):
+    """Runs the replay in a fresh process and returns its result dict.  publish_every = k > 0 (with map_resolution) also
+    publishes the map after every k-th scan through the resident store and the reference, 'publishes' rows as _publish_pair."""
     import tempfile
     params = params or YAML_PARAMS
     laser = laser or DEFAULT_LASER
@@ -153,7 +181,7 @@ def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpd
     fin, fout = os.path.join(d, f"in_{which}.npz"), os.path.join(d, f"out_{which}.npz")
     np.savez(fin, ranges=ranges, odom=odom, pkeys=np.array(list(params.keys())), pvals=np.array(list(params.values()), dtype=np.float64),
              lkeys=np.array(list(laser.keys())), lvals=np.array(list(laser.values()), dtype=np.float64), use_solver=int(use_solver),
-             map_resolution=float(map_resolution))
+             map_resolution=float(map_resolution), publish_every=int(publish_every))
     env = dict(os.environ)
     r = subprocess.run([sys.executable, os.path.abspath(__file__), which, fin, fout], capture_output=True, text=True, env=env)
     if r.returncode != 0:
@@ -182,10 +210,11 @@ def make_trajectory(seed: int, n_scans: int, step: float = 0.5):
 
 
 def localization_inprocess(which: str, map_ranges, map_odom, loc_ranges, loc_odom, params: dict, loc_params: dict, laser: dict,
-                           events, map_resolution: float = 0.0):
+                           events, map_resolution: float = 0.0, publish_every: int = 0):
     """Maps with Mapper::Process, then applies loc_params and localizes scan by scan as the localization node does.
     events: (step, kind, pose) with kind "process_near" (that step's scan goes through ProcessAgainstNodesNearBy at pose) or
-    "clear_localization_buffer" (Mapper::ClearLocalizationBuffer before that step's scan)."""
+    "clear_localization_buffer" (Mapper::ClearLocalizationBuffer before that step's scan).  publish_every as run_inprocess, over
+    the localization steps (the resident store holds the map's scans from the first publish on)."""
     L = _bind(which)
     if which == "b200":
         L.b200_shim_match_calls.restype = C.c_long
@@ -213,7 +242,7 @@ def localization_inprocess(which: str, map_ranges, map_odom, loc_ranges, loc_odo
     covs = np.full((n, 3, 3), np.nan)
     step_counts = np.zeros((n, 4), dtype=np.int32)
     step_seconds = np.zeros(n)
-    clear_counts = []
+    clear_counts, publishes = [], []
     for i in range(n):
         if i in clear:
             if L.krep_clear_localization_buffer(h) != 0:
@@ -238,6 +267,8 @@ def localization_inprocess(which: str, map_ranges, map_odom, loc_ranges, loc_odo
         before = st[0]
         L.krep_stats(h, st.ctypes.data_as(_DP))
         step_seconds[i] = st[0] - before
+        if publish_every and (i + 1) % publish_every == 0:
+            _publish_pair(L, h, map_resolution, i, publishes)
     L.krep_stats(h, st.ctypes.data_as(_DP))
     ids, scan_poses = _scans(L, h)
     ne = L.krep_edges(h, None, None, None, None, 0)
@@ -257,11 +288,13 @@ def localization_inprocess(which: str, map_ranges, map_odom, loc_ranges, loc_odo
                loc_match_calls=(int(L.b200_shim_match_calls()) - map_matches) if which == "b200" else 0)
     if map_resolution:
         _occupancy(L, h, map_resolution, out)
+    if publish_every:
+        out["publishes"] = np.array(publishes, dtype=np.float64).reshape(-1, 8)
     return out
 
 
 def run_localization(which: str, map_ranges, map_odom, loc_ranges, loc_odom, params=None, events=(), loc_params=None, laser=None,
-                     map_resolution=0.0, tmpdir=None):
+                     map_resolution=0.0, tmpdir=None, publish_every=0):
     """Maps map_* with Mapper::Process, then localizes loc_* with Mapper::ProcessLocalization (params updated by loc_params,
     LOCALIZATION_PARAMS by default), in a fresh process; events as localization_inprocess.  Returns per-step processed flags,
     published poses and covariances, graph sizes (mapper vertices, mapper edges, solver nodes, solver edges) and mapper seconds
@@ -280,7 +313,7 @@ def run_localization(which: str, map_ranges, map_odom, loc_ranges, loc_odom, par
              pkeys=np.array(list(params.keys())), pvals=np.array(list(params.values()), dtype=np.float64),
              qkeys=np.array(list(loc_params.keys())), qvals=np.array(list(loc_params.values()), dtype=np.float64),
              lkeys=np.array(list(laser.keys())), lvals=np.array(list(laser.values()), dtype=np.float64), events=ev,
-             map_resolution=float(map_resolution))
+             map_resolution=float(map_resolution), publish_every=int(publish_every))
     r = subprocess.run([sys.executable, os.path.abspath(__file__), f"localize-{which}", fin, fout], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"localization replay {which} failed:\n{r.stdout[-2000:]}\n{r.stderr[-2000:]}")
@@ -378,9 +411,11 @@ if __name__ == "__main__":
             loc_params = {str(k): float(v) for k, v in zip(z["qkeys"], z["qvals"])}
             events = [(int(e[0]), ("process_near", "clear_localization_buffer")[int(e[1])], e[2:]) for e in z["events"]]
             out = localization_inprocess(which[len("localize-"):], z["map_ranges"], z["map_odom"], z["loc_ranges"], z["loc_odom"],
-                                         params, loc_params, laser, events, float(z["map_resolution"]))
+                                         params, loc_params, laser, events, float(z["map_resolution"]),
+                                         int(z["publish_every"]) if "publish_every" in z.files else 0)
         else:
-            out = run_inprocess(which, z["ranges"], z["odom"], params, laser, bool(int(z["use_solver"])), float(z["map_resolution"]))
+            out = run_inprocess(which, z["ranges"], z["odom"], params, laser, bool(int(z["use_solver"])), float(z["map_resolution"]),
+                                int(z["publish_every"]) if "publish_every" in z.files else 0)
     finally:
         os.dup2(saved, 1)
     np.savez(fout, **out)

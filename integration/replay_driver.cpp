@@ -9,6 +9,7 @@
 #include <csignal>
 #include <cstdlib>
 #include <execinfo.h>
+#include <memory>
 #include <string>
 #include <unistd.h>
 
@@ -18,11 +19,16 @@
 
 using namespace karto;
 
+// defined by scan_matcher_b200.cpp, which only libreplay_b200.so links: without it, CorrectPoses calls cannot be counted
+extern "C" long b200_shim_correct_poses_calls() __attribute__((weak));
+
 namespace {
 struct Replay {
   Mapper mapper;
   solver_plugins::B200Solver * solver = nullptr;
   double process_seconds = 0.0;
+  std::unique_ptr<karto::b200::ResidentOccupancyMap> resident;   // krep_occupancy_resident's store
+  long corrections_seen = -1;
 };
 const char * kLaser = "laser0";
 
@@ -318,6 +324,33 @@ double krep_occupancy(void * rp, double resolution, int use_gpu, int info[3], do
   auto t0 = std::chrono::steady_clock::now();
   OccupancyGrid * g = use_gpu ? karto::b200::CreateOccupancyGridFromScans(v, resolution) : OccupancyGrid::CreateFromScans(v, resolution);
   const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  if (!g) return -1.0;
+  info[0] = g->GetWidth(); info[1] = g->GetHeight(); info[2] = g->GetWidthStep();
+  offset[0] = g->GetCoordinateConverter()->GetOffset().GetX();
+  offset[1] = g->GetCoordinateConverter()->GetOffset().GetY();
+  if (cells && cap >= static_cast<long>(g->GetDataSize())) std::memcpy(cells, g->GetDataPointer(), g->GetDataSize());
+  delete g;
+  return sec;
+}
+
+// the same map publish through karto::b200::ResidentOccupancyMap, whose scans stay on the device between calls: removed scans
+// are compacted out, new ones appended, and everything reloads after a MapperGraph::CorrectPoses (always, where the driver cannot
+// count those: libreplay_ref.so).  info / offset / cells as krep_occupancy; stats = {removed, appended, reloaded} of this publish,
+// device_ms = the build's device time.  Returns wall seconds, < 0 on failure.
+double krep_occupancy_resident(void * rp, double resolution, int info[3], double offset[2], unsigned char * cells, long cap, int stats[3],
+                               float * device_ms)
+{
+  Replay * r = static_cast<Replay *>(rp);
+  const LocalizedRangeScanVector v = processed_scans(r);
+  const long corrections = b200_shim_correct_poses_calls ? b200_shim_correct_poses_calls() : r->corrections_seen - 1;
+  const bool corrected = corrections != r->corrections_seen;
+  r->corrections_seen = corrections;
+  if (!r->resident) r->resident.reset(new karto::b200::ResidentOccupancyMap());
+  karto::b200::ResidentOccupancyMap::Stats st;
+  auto t0 = std::chrono::steady_clock::now();
+  OccupancyGrid * g = r->resident->Publish(v, resolution, corrected, &st, device_ms);
+  const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  if (stats) { stats[0] = st.removed; stats[1] = st.appended; stats[2] = st.reloaded; }
   if (!g) return -1.0;
   info[0] = g->GetWidth(); info[1] = g->GetHeight(); info[2] = g->GetWidthStep();
   offset[0] = g->GetCoordinateConverter()->GetOffset().GetX();

@@ -34,6 +34,7 @@ b200sm * handle_of(const ScanMatcher * m)
   return handles().at(m);
 }
 long g_match_calls = 0;
+long g_correct_poses_calls = 0;
 
 b200_scan to_scan(LocalizedRangeScan * s)
 {
@@ -52,6 +53,8 @@ inline LocalizedRangeScan * deref(LocalizedRangeScanMap::const_iterator it) { re
 }  // namespace
 
 extern "C" long b200_shim_match_calls() { return g_match_calls; }
+// MapperGraph::CorrectPoses calls so far: a resident map store (integration/occupancy_b200.hpp) reloads after each one
+extern "C" long b200_shim_correct_poses_calls() { return g_correct_poses_calls; }
 extern "C" long b200_shim_live_handles()
 {
   std::lock_guard<std::mutex> lock(handles_mutex());
@@ -116,6 +119,7 @@ ScanMatcher * ScanMatcher::Create(Mapper * pMapper, kt_double searchSize, kt_dou
 // bit-identical.
 void MapperGraph::CorrectPoses()
 {
+  ++g_correct_poses_calls;
   ScanSolver * pSolver = m_pMapper->m_pScanOptimizer;
   if (pSolver != NULL) {
     pSolver->Compute();

@@ -161,6 +161,7 @@ def lib():
     L.b200og_transform_scans.argtypes = [C.c_void_p, C.c_int32, C.c_int32, _DP, _DP, _DP]
     L.b200og_build_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(OgInfo)]
     L.b200og_scan_boxes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, _DP]
+    L.b200og_remove_scans.argtypes = [C.c_void_p, _IP, C.c_int32]
     _lib = L
     return L
 
@@ -651,6 +652,12 @@ class OccupancyGrid:
         out = np.zeros((max(int(count), 0), 4))
         _check(lib().b200og_scan_boxes(self._h, int(first), int(count), _dp(out)))
         return out
+
+    def RemoveScans(self, indices):
+        """Removes the scans at the given store indices (strictly increasing) and compacts the store on the device; the
+        survivors keep their order, stored boxes and the transformed state are kept"""
+        idx = np.ascontiguousarray(indices, dtype=np.int32).reshape(-1)
+        _check(lib().b200og_remove_scans(self._h, idx.ctypes.data_as(_IP), len(idx)))
 
     def GetWidth(self) -> int:
         return self.info.width

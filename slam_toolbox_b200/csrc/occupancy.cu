@@ -230,6 +230,41 @@ __global__ void __launch_bounds__(kOgThreads) k_og_box_union(const double * box,
   }
 }
 
+// Store compaction (b200og_remove_scans): scan k0 + k of the compacted store is old scan src[k].  One warp per surviving scan
+// copies its beams from the old offsets (old_start) to the new ones (new_start), its sensor position, and its box while the
+// old scan had one, into the second set of buffers.  Sources and destinations are different allocations, so no thread can
+// overwrite a value another one has not read yet.
+struct OgCompact {
+  const int32_t * src;
+  const int32_t * old_start;
+  const int32_t * new_start;
+  int32_t k0, count, nboxed;
+  const double * ranges;
+  const double * points;
+  const double * sensor;
+  const double * box;
+  double * ranges2;
+  double * points2;
+  double * sensor2;
+  double * box2;
+};
+
+__global__ void __launch_bounds__(kOgThreads) k_og_compact(OgCompact c)
+{
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * (kOgThreads / 32);
+  for (int64_t k = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); k < c.count; k += nwarps) {
+    const int32_t s = c.src[k], t = c.k0 + (int32_t)k;
+    const int32_t from = c.old_start[s], to = c.new_start[t], nb = c.old_start[s + 1] - from;
+    for (int32_t b = lane; b < nb; b += 32) {
+      c.ranges2[to + b] = c.ranges[from + b];
+      reinterpret_cast<double2 *>(c.points2)[to + b] = reinterpret_cast<const double2 *>(c.points)[from + b];
+    }
+    if (lane == 0) reinterpret_cast<double2 *>(c.sensor2)[t] = reinterpret_cast<const double2 *>(c.sensor)[s];
+    if (lane < 4 && s < c.nboxed) c.box2[4 * (size_t)t + lane] = c.box[4 * (size_t)s + lane];
+  }
+}
+
 // AddScan (Karto.h:6139-6182) + RayTrace (:6193-6229) + TraceLine (:4874-4927).
 // A warp takes 32 ADJACENT beams of one scan: every lane prepares its beam (the FP64 part: skip / clip rules, the
 // four world->grid conversions, the steep / direction swaps) and then runs the reference's own integer loop on it,
@@ -364,6 +399,7 @@ struct GrowBuf {
     p = q;
     cap = want;
   }
+  void swap(GrowBuf & o) { std::swap(p, o.p); std::swap(cap, o.cap); }
 };
 
 }  // namespace b200
@@ -383,6 +419,9 @@ struct b200og {
   GrowBuf<double> d_box;
   int32_t nboxed = 0;
   bool boxes_auth = false;
+  // compaction targets (b200og_remove_scans), swapped with the store's buffers after each compaction
+  GrowBuf<double> d_ranges2, d_points2, d_sensor2, d_box2;
+  GrowBuf<int32_t> d_start2, d_src;
   // staging (two pinned halves, filled while the other one is in flight)
   double * stage[2] = {nullptr, nullptr};
   cudaEvent_t stage_done[2] = {nullptr, nullptr};
@@ -630,6 +669,76 @@ int scan_boxes(b200og * h, int32_t first, int32_t count, double * boxes)
   return B200_OK;
 }
 
+int remove_scans(b200og * h, const int32_t * idx, int32_t n)
+{
+  const int32_t S = h->nscans();
+  if (n < 0 || (n > 0 && !idx)) { set_last_error("b200og_remove_scans: NULL indices or negative count"); return B200_ERR_INVALID_ARG; }
+  for (int32_t k = 0; k < n; ++k) {
+    if (idx[k] < 0 || idx[k] >= S) { set_last_error("b200og_remove_scans: index outside the store"); return B200_ERR_INVALID_ARG; }
+    if (k > 0 && idx[k] <= idx[k - 1]) {
+      set_last_error("b200og_remove_scans: indices not strictly increasing");
+      return B200_ERR_INVALID_ARG;
+    }
+  }
+  if (n == 0) return B200_OK;
+  // the new beam prefix, and the old index of every surviving scan from the first removed one on (those are the ones that move)
+  const int32_t k0 = idx[0], S2 = S - n;
+  std::vector<int32_t> src;
+  src.reserve((size_t)(S2 - k0));
+  for (int32_t s = k0 + 1, r = 1; s < S; ++s) {
+    if (r < n && idx[r] == s) { ++r; continue; }
+    src.push_back(s);
+  }
+  std::vector<int32_t> start(h->start.begin(), h->start.begin() + k0 + 1);
+  for (int32_t s : src) start.push_back(start.back() + (h->start[s + 1] - h->start[s]));
+  int32_t maxbeams = 0;
+  for (int32_t s = 0; s < S2; ++s) maxbeams = std::max(maxbeams, start[s + 1] - start[s]);
+  const int32_t nboxed = h->nboxed <= k0 ? h->nboxed
+                                         : k0 + (int32_t)(std::lower_bound(src.begin(), src.end(), h->nboxed) - src.begin());
+  h->last_ms = 0.f;
+  if (!src.empty()) {
+    cudaStream_t st = h->stream;
+    const size_t keep = (size_t)start[k0], nbeams = (size_t)start[S2], kbox = (size_t)std::min(k0, h->nboxed);
+    const int32_t count = (int32_t)src.size();
+    h->d_ranges2.ensure(nbeams, 0, st);
+    h->d_points2.ensure(2 * nbeams, 0, st);
+    h->d_sensor2.ensure(2 * (size_t)S2, 0, st);
+    h->d_start2.ensure((size_t)S2 + 1, 0, st);
+    h->d_src.ensure((size_t)count, 0, st);
+    if (h->nboxed) h->d_box2.ensure(4 * (size_t)nboxed, 0, st);
+    // the scans before the first removed one keep their offsets: plain copies into the second buffers
+    if (keep) {
+      B200_CUDA(cudaMemcpyAsync(h->d_ranges2.p, h->d_ranges.p, keep * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      B200_CUDA(cudaMemcpyAsync(h->d_points2.p, h->d_points.p, 2 * keep * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    }
+    if (k0) B200_CUDA(cudaMemcpyAsync(h->d_sensor2.p, h->d_sensor.p, 2 * (size_t)k0 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (kbox) B200_CUDA(cudaMemcpyAsync(h->d_box2.p, h->d_box.p, 4 * kbox * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(h->d_start2.p, start.data(), start.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(h->d_src.p, src.data(), src.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    OgCompact c{h->d_src.p, h->d_start.p, h->d_start2.p, k0, count, h->nboxed, h->d_ranges.p, h->d_points.p, h->d_sensor.p,
+                h->d_box.p, h->d_ranges2.p, h->d_points2.p, h->d_sensor2.p, h->d_box2.p};
+    const int nb = (int)std::min<int64_t>(((int64_t)count + kOgThreads / 32 - 1) / (kOgThreads / 32), (int64_t)h->sms * 8);
+    B200_CUDA(cudaEventRecord(h->ev0, st));
+    k_og_compact<<<nb, kOgThreads, 0, st>>>(c);
+    B200_CUDA(cudaGetLastError());
+    ++h->launches;
+    B200_CUDA(cudaEventRecord(h->ev1, st));
+    B200_CUDA(cudaStreamSynchronize(st));   // start and src are released on return
+    B200_CUDA(cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+    h->d_ranges.swap(h->d_ranges2);
+    h->d_points.swap(h->d_points2);
+    h->d_sensor.swap(h->d_sensor2);
+    h->d_start.swap(h->d_start2);
+    if (h->nboxed) h->d_box.swap(h->d_box2);
+  }
+  // removing only trailing scans moves nothing: the device prefix up to the new end is unchanged
+  h->start.swap(start);
+  h->maxbeams = maxbeams;
+  h->nboxed = nboxed;
+  h->built = false;
+  return B200_OK;
+}
+
 int build(b200og * h, int32_t first, int32_t count, b200og_info * info)
 {
   if (info) std::memset(info, 0, sizeof(*info));
@@ -818,6 +927,14 @@ int b200og_scan_boxes(b200og * h, int32_t first, int32_t count, double * boxes)
   B200_GUARD_BEGIN
   if (!h) return B200_ERR_INVALID_ARG;
   return scan_boxes(h, first, count, boxes);
+  B200_GUARD_END
+}
+
+int b200og_remove_scans(b200og * h, const int32_t * indices, int32_t n)
+{
+  B200_GUARD_BEGIN
+  if (!h) { set_last_error("b200og_remove_scans: NULL handle"); return B200_ERR_INVALID_ARG; }
+  return remove_scans(h, indices, n);
   B200_GUARD_END
 }
 
