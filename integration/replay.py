@@ -57,6 +57,7 @@ def _bind(which: str):
     L.krep_process_localization.argtypes = [C.c_void_p, _DP, C.c_int, _DP, C.c_int, _DP, _DP]
     L.krep_process_near.argtypes = [C.c_void_p, _DP, C.c_int, _DP, C.c_int, _DP, _DP, _DP]
     L.krep_clear_localization_buffer.argtypes = [C.c_void_p]
+    L.krep_remove_node.argtypes = [C.c_void_p, C.c_int]
     L.krep_num_scans.argtypes = [C.c_void_p]
     L.krep_poses.argtypes = [C.c_void_p, _DP, C.POINTER(C.c_int)]
     L.krep_stats.argtypes = [C.c_void_p, _DP]
@@ -105,6 +106,49 @@ def _solver_graph(L, h, cap: int):
     return gn, gids[:min(gn, cap)][order], gposes[:min(gn, cap)][order]
 
 
+def _edges(L, h):
+    """The mapper's graph edges (krep_edges, insertion order): source ids, target ids, pose differences, covariances."""
+    ne = L.krep_edges(h, None, None, None, None, 0)
+    src, dst = np.zeros(max(ne, 1), dtype=np.int32), np.zeros(max(ne, 1), dtype=np.int32)
+    diff, cov = np.zeros((max(ne, 1), 3)), np.zeros((max(ne, 1), 3, 3))
+    L.krep_edges(h, src.ctypes.data_as(C.POINTER(C.c_int)), dst.ctypes.data_as(C.POINTER(C.c_int)), diff.ctypes.data_as(_DP),
+                 cov.ctypes.data_as(_DP), ne)
+    return src[:ne], dst[:ne], diff[:ne], cov[:ne]
+
+
+def lifelong_candidates(ids, src, dst, buffer: int):
+    """The scans lifelong mode may remove (src/experimental/slam_toolbox_lifelong.cpp:271-278, 313), sorted: not ids 0 and 1,
+    at least `buffer` (scan_buffer_size) ids older than the newest scan, and with two or more graph edges."""
+    ids = np.asarray(ids)
+    if len(ids) == 0:
+        return ids
+    deg = {int(i): 0 for i in ids}
+    for a, b in zip(np.asarray(src).tolist(), np.asarray(dst).tolist()):
+        deg[a] += 1
+        deg[b] += 1
+    newest = int(ids.max())
+    return np.array(sorted(i for i, d in deg.items() if i > 1 and newest - i >= buffer and d >= 2), dtype=np.int64)
+
+
+def _remove_node(L, h, step: int, nid: int, buffer: int, log: list):
+    """krep_remove_node on nid, or (nid < 0) on a lifelong candidate picked from the mapper's edges by a generator seeded with
+    the step.  Appends [step, id, its edges, its index among the stored scans, scans, return code, mapper vertices, mapper
+    edges, solver nodes, solver edges, solver node set == mapper scan set]."""
+    ids, _ = _scans(L, h)
+    src, dst, _, _ = _edges(L, h)
+    if nid < 0:
+        cand = lifelong_candidates(ids, src, dst, buffer)
+        nid = int(cand[np.random.default_rng(step).integers(len(cand))]) if len(cand) else 0
+    deg = int(np.sum(src == nid) + np.sum(dst == nid))
+    pos = int(np.searchsorted(ids, nid)) if nid in ids else -1
+    rc = L.krep_remove_node(h, nid)
+    counts = (C.c_int * 4)()
+    L.krep_counts(h, counts)
+    after, _ = _scans(L, h)
+    _, gids, _ = _solver_graph(L, h, len(after) + 16)
+    log.append([step, nid, deg, pos, len(ids), rc] + counts[:] + [int(np.array_equal(gids, np.sort(after)))])
+
+
 def _occupancy(L, h, map_resolution: float, out: dict):
     """The map-publish step over the mapper's scans: reference CPU build and the b200og binding, same process."""
     for tag, gpu in (("cpu", 0), ("gpu", 1)):
@@ -142,17 +186,25 @@ def _publish_pair(L, h, map_resolution: float, step: int, log: list):
 
 
 def run_inprocess(which: str, ranges: np.ndarray, odom: np.ndarray, params: dict, laser: dict, use_solver: bool = True,
-                  map_resolution: float = 0.0, publish_every: int = 0):
+                  map_resolution: float = 0.0, publish_every: int = 0, events=()):
     L = _bind(which)
     h = _create(L, laser, params, use_solver)
     ranges = np.ascontiguousarray(ranges, dtype=np.float64)
     odom = np.ascontiguousarray(odom, dtype=np.float64)
-    kept, publishes = [], []
+    kept, publishes, removals = [], [], []
+    buffer = int(params.get("scan_buffer_size", YAML_PARAMS["scan_buffer_size"]))
     for i in range(len(ranges)):
         if L.krep_process(h, ranges[i].ctypes.data_as(_DP), ranges.shape[1], odom[i].ctypes.data_as(_DP), i):
             kept.append(i)
         if publish_every and (i + 1) % publish_every == 0:
             _publish_pair(L, h, map_resolution, i, publishes)
+        for ev in events:
+            if ev[0] != i:
+                continue
+            if ev[1] == "remove_node":
+                _remove_node(L, h, i, int(ev[2]), buffer, removals)
+            else:
+                _publish_pair(L, h, map_resolution, i, publishes)
     _, poses = _scans(L, h)
     n = len(poses)
     st = np.zeros(5)
@@ -166,14 +218,22 @@ def run_inprocess(which: str, ranges: np.ndarray, odom: np.ndarray, params: dict
                process_seconds=st[0], solver_computes=int(st[1]), solver_ms=st[2], edges=int(st[3]), scans=int(st[4]), match_calls=matches)
     if map_resolution:
         _occupancy(L, h, map_resolution, out)
-    if publish_every:
+    if publish_every or events:
         out["publishes"] = np.array(publishes, dtype=np.float64).reshape(-1, 8)
+    if events:
+        out["removals"] = np.array(removals, dtype=np.int64).reshape(-1, 11)
+        out["edge_src"], out["edge_dst"], out["edge_diff"], out["edge_cov"] = _edges(L, h)
+        out["scan_ids"] = _scans(L, h)[0]
     return out
 
 
-def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpdir=None, map_resolution=0.0, publish_every=0):
+def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpdir=None, map_resolution=0.0, publish_every=0,
+        events=()):
     """Runs the replay in a fresh process and returns its result dict.  publish_every = k > 0 (with map_resolution) also
-    publishes the map after every k-th scan through the resident store and the reference, 'publishes' rows as _publish_pair."""
+    publishes the map after every k-th scan through the resident store and the reference, 'publishes' rows as _publish_pair.
+    events: after step i's scan, in list order, (i, "remove_node", id) removes a scan as lifelong mode does (krep_remove_node;
+    id < 0 picks one of lifelong_candidates, see _remove_node; 'removals' rows) and (i, "publish") publishes as
+    publish_every does.  With events the result also holds the mapper's final edges and scan ids."""
     import tempfile
     params = params or YAML_PARAMS
     laser = laser or DEFAULT_LASER
@@ -181,7 +241,8 @@ def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpd
     fin, fout = os.path.join(d, f"in_{which}.npz"), os.path.join(d, f"out_{which}.npz")
     np.savez(fin, ranges=ranges, odom=odom, pkeys=np.array(list(params.keys())), pvals=np.array(list(params.values()), dtype=np.float64),
              lkeys=np.array(list(laser.keys())), lvals=np.array(list(laser.values()), dtype=np.float64), use_solver=int(use_solver),
-             map_resolution=float(map_resolution), publish_every=int(publish_every))
+             map_resolution=float(map_resolution), publish_every=int(publish_every),
+             events=np.array([[e[0], e[1] == "remove_node", e[2] if len(e) > 2 else -1] for e in events], dtype=np.int64).reshape(-1, 3))
     env = dict(os.environ)
     r = subprocess.run([sys.executable, os.path.abspath(__file__), which, fin, fout], capture_output=True, text=True, env=env)
     if r.returncode != 0:
@@ -271,18 +332,14 @@ def localization_inprocess(which: str, map_ranges, map_odom, loc_ranges, loc_odo
             _publish_pair(L, h, map_resolution, i, publishes)
     L.krep_stats(h, st.ctypes.data_as(_DP))
     ids, scan_poses = _scans(L, h)
-    ne = L.krep_edges(h, None, None, None, None, 0)
-    src, dst = np.zeros(max(ne, 1), dtype=np.int32), np.zeros(max(ne, 1), dtype=np.int32)
-    diff, ecov = np.zeros((max(ne, 1), 3)), np.zeros((max(ne, 1), 3, 3))
-    L.krep_edges(h, src.ctypes.data_as(C.POINTER(C.c_int)), dst.ctypes.data_as(C.POINTER(C.c_int)), diff.ctypes.data_as(_DP),
-                 ecov.ctypes.data_as(_DP), ne)
+    src, dst, diff, ecov = _edges(L, h)
     gn, gids, gposes = _solver_graph(L, h, len(ids) + 16)
     nc = L.krep_solver_computes(h, None, None, 0)
     cms, cup = np.zeros(max(nc, 1)), np.zeros(max(nc, 1), dtype=np.int32)
     L.krep_solver_computes(h, cms.ctypes.data_as(_DP), cup.ctypes.data_as(C.POINTER(C.c_int)), nc)
     out = dict(flags=flags, poses=poses, covs=covs, step_counts=step_counts, step_seconds=step_seconds, map_counts=map_counts,
                clear_counts=np.array(clear_counts, dtype=np.int32).reshape(-1, 5), scan_ids=ids, scan_poses=scan_poses,
-               edge_src=src[:ne], edge_dst=dst[:ne], edge_diff=diff[:ne], edge_cov=ecov[:ne], graph_nodes=gn, graph_ids=gids,
+               edge_src=src, edge_dst=dst, edge_diff=diff, edge_cov=ecov, graph_nodes=gn, graph_ids=gids,
                graph_poses=gposes, map_computes=map_computes, map_seconds=map_seconds, loc_seconds=st[0] - map_seconds,
                compute_ms=cms[:nc], compute_uploaded=cup[:nc], map_match_calls=map_matches,
                loc_match_calls=(int(L.b200_shim_match_calls()) - map_matches) if which == "b200" else 0)
@@ -414,8 +471,9 @@ if __name__ == "__main__":
                                          params, loc_params, laser, events, float(z["map_resolution"]),
                                          int(z["publish_every"]) if "publish_every" in z.files else 0)
         else:
+            events = [(int(e[0]), "remove_node", int(e[2])) if e[1] else (int(e[0]), "publish") for e in z["events"]]
             out = run_inprocess(which, z["ranges"], z["odom"], params, laser, bool(int(z["use_solver"])), float(z["map_resolution"]),
-                                int(z["publish_every"]) if "publish_every" in z.files else 0)
+                                int(z["publish_every"]), events)
     finally:
         os.dup2(saved, 1)
     np.savez(fout, **out)

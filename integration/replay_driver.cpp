@@ -227,6 +227,37 @@ int krep_clear_localization_buffer(void * rp)
   return 0;
 }
 
+// LifelongSlamToolbox::removeFromSlamGraph (src/experimental/slam_toolbox_lifelong.cpp:332-344) on the scan with this unique id:
+// Mapper::RemoveNodeFromGraph (its edges leave the graph and the solver, then the node), the sensor manager's RemoveScan,
+// then the vertex lets go of the scan and both are freed (the mapper owns processed scans, as in the localization calls).
+// Refuses (-1, nothing done) what lifelong mode never removes and the mapper cannot take: ids 0 and 1, ids within
+// scan_buffer_size of the newest scan (the running buffer and the last scan are among those), unknown ids, and any
+// removal without a solver (RemoveNodeFromGraph calls it unchecked).  0 on success.
+int krep_remove_node(void * rp, int unique_id)
+{
+  Replay * r = static_cast<Replay *>(rp);
+  MapperSensorManager * sm = r->mapper.GetMapperSensorManager();
+  MapperGraph * g = r->mapper.GetGraph();
+  if (!r->solver || !sm || !g || unique_id == 0 || unique_id == 1) return -1;
+  const LocalizedRangeScanVector v = processed_scans(r);
+  if (v.empty() || v.back()->GetUniqueId() - unique_id < r->mapper.getParamScanBufferSize()) return -1;
+  LocalizedRangeScan * scan = nullptr;
+  for (LocalizedRangeScan * s : v)
+    if (s->GetUniqueId() == unique_id) scan = s;
+  if (!scan) return -1;
+  const auto byname = g->GetVertices().find(scan->GetSensorName());
+  if (byname == g->GetVertices().end()) return -1;
+  const auto it = byname->second.find(scan->GetStateId());
+  if (it == byname->second.end() || it->second->GetObject() != scan) return -1;
+  Vertex<LocalizedRangeScan> * vertex = it->second;
+  if (!r->mapper.RemoveNodeFromGraph(vertex)) return -1;
+  sm->RemoveScan(scan);
+  vertex->RemoveObject();
+  delete vertex;
+  delete scan;
+  return 0;
+}
+
 int krep_num_scans(void * rp) { return static_cast<int>(processed_scans(static_cast<Replay *>(rp)).size()); }
 
 // corrected poses (after all loop closures) of the scans the mapper holds, in processing order; ids (if not NULL) receives

@@ -68,9 +68,9 @@ def main():
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_dogleg_cfg4.json"))
     ap.add_argument("--reps", type=int, default=3)
     args = ap.parse_args()
-    # under dogleg the Gauss-Newton solve runs to pcg_tolerance / 10 (pose_graph.cu, kDlPcgTolFactor)
+    # under dogleg the Gauss-Newton solve runs to pcg_tolerance / 100 (pose_graph.cu, kDlPcgTolFactor)
     result = dict(card=card(), graph="synth.make_pose_graph(0, 10000, 40000)", pcg_tolerance_default=1e-9,
-                  dogleg_gauss_newton_tolerance="pcg_tolerance / 10", rows=[], sweep=[])
+                  dogleg_gauss_newton_tolerance="pcg_tolerance / 100", rows=[], sweep=[])
     for sig in ((0.03, 0.01), (0.05, 0.02)):
         g = synth.make_pose_graph(0, 10000, 40000, sigma_xy=sig[0], sigma_th=sig[1])
         for name, kw in STRATEGIES.items():
