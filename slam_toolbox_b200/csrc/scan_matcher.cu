@@ -529,6 +529,13 @@ int32_t device_offset(int32_t off, int data_size)
   return off;
 }
 
+void device_plan(const CorrPlan & pl, const GridGeom & g, int32_t * offsets, int32_t * posidx)
+{
+  for (size_t i = 0; i < (size_t)pl.nA * pl.n; ++i) offsets[i] = device_offset(pl.offsets[i], g.data_size);
+  for (int y = 0; y < pl.nY; ++y)
+    for (int x = 0; x < pl.nX; ++x) posidx[(size_t)y * pl.nX + x] = pl.xs[x] + pl.ys[y] * g.stride;
+}
+
 // ScanMatcher::CorrelateScan's reduction (M.cpp:775-862) + both covariance routines, in FP64 on the
 // host, from the device's integer volume. sums index = (y*nX + x)*nA + a.
 double host_epilogue(const b200sm_params & prm, const GridGeom & geom, int probs_side, const CorrPlan & pl,
@@ -695,15 +702,13 @@ static const int32_t * device_volume(b200sm * h, const CorrPlan & pl)
   h->ensure_stream();
   h->h_sums.reserve(total);
   if (pl.n == 0) { std::memset(h->h_sums.p, 0, total * sizeof(int32_t)); return h->h_sums.p; }
-  if ((size_t)pl.n * sizeof(int32_t) > 200 * 1024) {
+  if ((size_t)pl.n * sizeof(int32_t) > kLookupSmemBytes) {
     set_last_error("scan has too many readings for the shared-memory lookup row");
     throw CudaFail{B200_ERR_UNSUPPORTED};
   }
   const size_t noff = (size_t)pl.nA * pl.n;
   h->h_stage_i.reserve(noff + P);
-  for (size_t i = 0; i < noff; ++i) h->h_stage_i.p[i] = device_offset(pl.offsets[i], g.data_size);
-  for (int y = 0; y < pl.nY; ++y)
-    for (int x = 0; x < pl.nX; ++x) h->h_stage_i.p[noff + (size_t)y * pl.nX + x] = pl.xs[x] + pl.ys[y] * g.stride;
+  device_plan(pl, g, h->h_stage_i.p, h->h_stage_i.p + noff);
   h->d_offsets.reserve(noff + P);
   h->d_sums.reserve(total);
   B200_CUDA(cudaMemcpyAsync(h->d_offsets.p, h->h_stage_i.p, (noff + P) * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
@@ -864,6 +869,9 @@ int b200sm_create(const b200sm_params * params, b200sm ** out)
   if (rc != B200_OK) return rc;
   require_device();
   h->ensure_stream();
+  int dev = 0;
+  B200_CUDA(cudaGetDevice(&dev));
+  B200_CUDA(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, dev));
   *out = h.release();
   return B200_OK;
   B200_GUARD_END

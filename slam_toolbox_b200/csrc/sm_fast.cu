@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(kFastThreads, 1) k_sweep_fast(SweepDev d, Fast
       for (int wi = warp; wi < nA * f.xtiles; wi += nwarps) {
         const int a = wi / f.xtiles, xt = wi - a * f.xtiles;
         const int32_t * cs = f.cls_start + ((size_t)q * nA + a) * 33 + ph * 8;
-        const int32_t * es = f.edge_start + ((size_t)q * nA + a) * 17 + ph * 4;
+        const int32_t * es = f.edge_start + ((size_t)q * nA + a) * 16 + ph * 4;
         const uint32_t base = (uint32_t)((y_l * kSubPitchW + 4 * xt + j_l) * 4);
         int32_t * Arow = A + a * P;
         for (int m = 0; m < 4; ++m) {
@@ -279,7 +279,7 @@ bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   const CorrPlan & p0 = S.plans[0];
   const int nX = p0.nX, nY = p0.nY, nA = p0.nA, n = p0.n, nq = S.nq;
   auto bail = [&](int why) { S.fast_refusal = why; return false; };
-  if (g.order_dependent) return bail(1);
+  if (const int why = parity_refusal(g, S.plans)) return bail(why);
   if (nY > 8 * kFastRowTiles || (g.stride & 1) || nX * nY > 3 * kFastThreads) return bail(2);
   if (g.stride / 2 > kSubPitchW * 4 - 16) return bail(3);   // sub-grid row + the 3-word overhang must fit the pitch
   const int xtiles = (nX + 3 + 15) / 16;
@@ -289,95 +289,59 @@ bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   const size_t smem = (size_t)sub_rows * kSubPitchW * 4 + (size_t)nA * nX * nY * 4;
   if (smem > 227 * 1024 - 1024) return bail(4);
   if ((size_t)5 * nX * nY * sizeof(double) > (size_t)sub_rows * kSubPitchW * 4) return bail(5);   // epilogue scratch reuses S
-  std::vector<int32_t> cls_start((size_t)nq * nA * 33), slow, slow_start((size_t)nq * (nA + 1));
+  std::vector<int32_t> cls_start((size_t)nq * nA * 33);
   std::vector<uint16_t> beams, mult;
-  std::vector<int32_t> wrap2, wrap2_start((size_t)nq * nA * 4 + 1);
-  std::vector<int32_t> edge, edge_start((size_t)nq * nA * 17);
-  int n_edge = 0;
+  BeamLists lists;
   beams.reserve((size_t)nq * nA * n);
   mult.reserve((size_t)nq * nA * n);
   // one angle's lists, built independently (one host-pool task per angle), then concatenated in angle order: its beam classes
   // (one band: stage = phase) and the FAST descriptors
   struct AngleLists {
-    BeamClasses cls;
     std::vector<uint16_t> beams, mult;
     int32_t cs[33];                          // relative to the angle's first descriptor
   };
+  std::vector<BeamClasses> cls(nA);
   std::vector<AngleLists> al(nA);
   for (int q = 0; q < nq; ++q) {
     const CorrPlan & pl = S.plans[q];
-    for (int k = 1; k < nX; ++k) if (pl.xs[k] != pl.xs[0] + 2 * k) return bail(6);   // coarse step must be exactly 2 cells
-    for (int k = 1; k < nY; ++k) if (pl.ys[k] != pl.ys[0] + 2 * k) return bail(7);
     auto one_angle = [&](int a) {
       AngleLists & L = al[a];
-      classify_beams(g, pl, a, kSubPitchW, sub_rows, 1, L.cls);
+      classify_beams(g, pl, a, kSubPitchW, sub_rows, 1, cls[a]);
       L.beams.clear(); L.mult.clear();
       for (int k = 0; k < 16; ++k) {
-        std::vector<uint16_t> & gk = L.cls.fast[k];
+        std::vector<uint16_t> & gk = cls[a].fast[k];
         std::sort(gk.begin(), gk.end());
         L.cs[2 * k] = (int32_t)L.beams.size();
-        // run-length encode: beams that land in the same cell share a descriptor. Entries with multiplicity >= 3
-        // go to the group's multi list (one load, fields multiplied), provided the whole group fits one flush.
-        const bool dedup = !h->no_dedup && gk.size() <= (size_t)kFastChunk;
+        // beams that land in the same cell share a descriptor: runs of >= 3 go to the group's multi list (one load, fields
+        // multiplied), provided the whole group fits one flush
         std::vector<std::pair<uint16_t, uint16_t>> multi;
-        for (size_t i = 0; i < gk.size();) {
-          size_t j = i;
-          while (j < gk.size() && gk[j] == gk[i]) ++j;
-          const size_t cnt = j - i;
-          if (dedup && cnt >= 3) {
-            multi.emplace_back(gk[i], (uint16_t)cnt);
-          } else {
-            for (size_t t = 0; t < cnt; ++t) { L.beams.push_back(gk[i]); L.mult.push_back(1); }
-          }
-          i = j;
-        }
+        encode_runs(gk, 3, !h->no_dedup && gk.size() <= (size_t)kFastChunk, L.beams, multi);
+        L.mult.resize(L.beams.size(), 1);
         L.cs[2 * k + 1] = (int32_t)L.beams.size();
         for (auto & mk : multi) { L.beams.push_back(mk.first); L.mult.push_back(mk.second); }
       }
       L.cs[32] = (int32_t)L.beams.size();
     };
     host_parallel_for(nA, one_angle);
+    append_beam_lists(cls, 4, lists);
     for (int a = 0; a < nA; ++a) {
       const AngleLists & L = al[a];
-      slow_start[(size_t)q * (nA + 1) + a] = (int32_t)slow.size();
-      slow.insert(slow.end(), L.cls.far.begin(), L.cls.far.end());
-      n_edge += L.cls.n_edge;
-      for (int k = 0; k < 4; ++k) {
-        wrap2_start[((size_t)q * nA + a) * 4 + k] = (int32_t)wrap2.size();
-        wrap2.insert(wrap2.end(), L.cls.wrap2[k].begin(), L.cls.wrap2[k].end());
-      }
-      for (int k = 0; k < 16; ++k) {
-        edge_start[((size_t)q * nA + a) * 17 + k] = (int32_t)edge.size();
-        edge.insert(edge.end(), L.cls.edge[k].begin(), L.cls.edge[k].end());
-      }
-      edge_start[((size_t)q * nA + a) * 17 + 16] = (int32_t)edge.size();
       int32_t * cs = &cls_start[((size_t)q * nA + a) * 33];
       const int32_t base = (int32_t)beams.size();
       for (int k = 0; k < 33; ++k) cs[k] = base + L.cs[k];
       beams.insert(beams.end(), L.beams.begin(), L.beams.end());
       mult.insert(mult.end(), L.mult.begin(), L.mult.end());
     }
-    slow_start[(size_t)q * (nA + 1) + nA] = (int32_t)slow.size();
   }
-  wrap2_start[(size_t)nq * nA * 4] = (int32_t)wrap2.size();
-  // slow_start must be relative to one array: it is (single vector `slow`)
-  h2d(S.d_fast_cls, cls_start.data(), cls_start.size(), st);
+  S.h2d(S.d_fast_cls, cls_start.data(), cls_start.size(), st);
   S.d_fast_beams.reserve(std::max<size_t>(beams.size(), 1) + 8);
-  sweep_stage_h2d(S.d_fast_beams.p, beams.data(), beams.size() * sizeof(uint16_t), st);
+  S.stage(S.d_fast_beams.p, beams.data(), beams.size() * sizeof(uint16_t), st);
   S.d_fast_mult.reserve(std::max<size_t>(mult.size(), 1) + 8);
-  sweep_stage_h2d(S.d_fast_mult.p, mult.data(), mult.size() * sizeof(uint16_t), st);
-  slow.push_back(0);
-  wrap2.push_back(0);
-  edge.push_back(0);
-  h2d(S.d_edge, edge.data(), edge.size(), st);
-  h2d(S.d_edge_start, edge_start.data(), edge_start.size(), st);
-  h2d(S.d_wrap2, wrap2.data(), wrap2.size(), st);
-  h2d(S.d_wrap2_start, wrap2_start.data(), wrap2_start.size(), st);
-  h2d(S.d_slow, slow.data(), slow.size(), st);
-  h2d(S.d_slow_start, slow_start.data(), slow_start.size(), st);
+  S.stage(S.d_fast_mult.p, mult.data(), mult.size() * sizeof(uint16_t), st);
+  upload_beam_lists(lists, S, st);
+  S.beam_counts[0] = (int32_t)beams.size();   // this kernel counts FAST descriptors, not beams
   S.fast.enabled = 1;
   S.fast_refusal = 0;
-  S.beam_counts[0] = (int32_t)beams.size(); S.beam_counts[1] = n_edge; S.beam_counts[2] = (int32_t)slow.size() - 1;
   S.fast.sub_rows = sub_rows;
   S.fast.xtiles = xtiles;
   S.fast.beams = S.d_fast_beams.p;
@@ -390,12 +354,7 @@ bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   S.fast.wrap2_start = S.d_wrap2_start.p;
   S.fast.slow_start = S.d_slow_start.p;
   S.fast_smem = smem;
-  {
-    int dev = 0, sms = 132;
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    S.fast_blocks = std::min(S.npairs, sms);
-  }
+  S.fast_blocks = std::min(S.npairs, h->sms);
   return true;
 }
 

@@ -342,26 +342,22 @@ void SweepHost::release()
   uploaded = ran = false;
 }
 
-static thread_local int64_t * g_h2d_counter = nullptr;
-
 // Host -> device copy of a small table through the sweep's pinned arena: the source may be reused or freed as soon as this
 // returns and nothing blocks, so the host keeps building tables while the candidate points are still in flight.
-static thread_local SweepHost * g_arena_owner = nullptr;
-void sweep_stage_h2d(void * dst, const void * src, size_t bytes, cudaStream_t s)
+void SweepHost::stage(void * dst, const void * src, size_t bytes, cudaStream_t s)
 {
   if (!bytes) return;
-  SweepHost * S = g_arena_owner;
   const size_t need = (bytes + 63) & ~(size_t)63;
-  if (S && S->arena_used + need <= S->arena.cap) {
-    unsigned char * stage = S->arena.p + S->arena_used;
-    S->arena_used += need;
-    std::memcpy(stage, src, bytes);
-    B200_CUDA(cudaMemcpyAsync(dst, stage, bytes, cudaMemcpyHostToDevice, s));
+  if (arena_used + need <= arena.cap) {
+    unsigned char * slot = arena.p + arena_used;
+    arena_used += need;
+    std::memcpy(slot, src, bytes);
+    B200_CUDA(cudaMemcpyAsync(dst, slot, bytes, cudaMemcpyHostToDevice, s));
   } else {
     B200_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s));
     B200_CUDA(cudaStreamSynchronize(s));   // arena exhausted: plain copy, the source may go away after return
   }
-  if (g_h2d_counter) *g_h2d_counter += (int64_t)bytes;
+  h2d_bytes += (int64_t)bytes;
 }
 
 static GridGeom geom_for_query(const b200sm * h, const b200_scan * q)
@@ -383,15 +379,12 @@ static void coarse_search(const b200sm * h, double off[2], double res[2])
   res[0] = res[1] = 2 * r;                 // M.cpp:584-585
 }
 
-
-// shared memory the generic kernel may fill with lookup rows; a query needs at least one row (n <= 51,200 readings)
-constexpr size_t kGenericTableBytes = 200 * 1024;
 // whole angle rows of the lookup table per slice of the generic kernel: all nA when the table fits (one slice, staged once
 // per query), else as many as fit
 static int generic_slice_rows(int nA, int n)
 {
   const size_t row = (size_t)n * sizeof(int32_t);
-  return (int)std::min<size_t>((size_t)nA, kGenericTableBytes / row);
+  return (int)std::min<size_t>((size_t)nA, kLookupSmemBytes / row);
 }
 
 static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b200_scan * scans, int nscans,
@@ -411,7 +404,6 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   for (int i = 0; i < 8; ++i) if (i != 5) S.tile_info[i] = 0;
   std::fill(S.tile_stats, S.tile_stats + 8, 0);
   std::fill(S.tile_layout, S.tile_layout + 4, 0);
-  g_h2d_counter = &S.h2d_bytes;
   if (!queries || nq <= 0 || !scans || nscans <= 0 || !chain_start || nchains <= 0) {
     set_last_error("sweep: empty or NULL input");
     return B200_ERR_INVALID_ARG;
@@ -433,7 +425,6 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   cudaStream_t st = h->stream;
   const GridGeom & g0 = h->g;
   B200_CUDA(cudaStreamSynchronize(st));   // copies of the previous upload are done: its staging arena can be reused
-  g_arena_owner = &S;
   S.arena_used = S.arena.cap;             // nothing staged until the arena is sized (after the plans, below)
 
   // ---- candidate scans first: their 17 KB/scan copy runs while the host builds the per-query tables ----
@@ -486,7 +477,7 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
     S.arena.reserve((size_t)nq * per_query + lists + (size_t)npairs * items * 8);
     S.arena_used = 0;
   }
-  if ((size_t)n * sizeof(int32_t) > kGenericTableBytes) {
+  if ((size_t)n * sizeof(int32_t) > kLookupSmemBytes) {
     set_last_error("sweep: one lookup row of the query does not fit shared memory (more than 51,200 readings per query)");
     return B200_ERR_UNSUPPORTED;
   }
@@ -506,14 +497,9 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   {
     const size_t no = (size_t)nq * nA * n, np = (size_t)nq * P;
     S.h_i.reserve(no + np);
-    for (int q = 0; q < nq; ++q) {
-      const CorrPlan & pl = S.plans[q];
-      for (size_t i = 0; i < (size_t)nA * n; ++i) S.h_i.p[(size_t)q * nA * n + i] = device_offset(pl.offsets[i], g0.data_size);
-      for (int y = 0; y < nY; ++y)
-        for (int x = 0; x < nX; ++x) S.h_i.p[no + (size_t)q * P + (size_t)y * nX + x] = pl.xs[x] + pl.ys[y] * g0.stride;
-    }
-    h2d(S.d_offsets, S.h_i.p, no, st);
-    h2d(S.d_posidx, S.h_i.p + no, np, st);
+    for (int q = 0; q < nq; ++q) device_plan(S.plans[q], g0, S.h_i.p + (size_t)q * nA * n, S.h_i.p + no + (size_t)q * P);
+    S.h2d(S.d_offsets, S.h_i.p, no, st);
+    S.h2d(S.d_posidx, S.h_i.p + no, np, st);
     // doubles: qgeom[4], center[3], then 6 arrays of nX/nY, angpen
     const size_t per = 4 + 3 + 3 * (size_t)nX + 3 * (size_t)nY + nA;
     S.h_d.reserve(per * nq);
@@ -530,7 +516,7 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
       for (int y = 0; y < nY; ++y) { yrel[(size_t)q * nY + y] = pl.yrel[y]; newy[(size_t)q * nY + y] = pl.newy[y]; sqy[(size_t)q * nY + y] = pl.sqy[y]; }
       for (int a = 0; a < nA; ++a) angpen[(size_t)q * nA + a] = pl.angpen[a];
     }
-    h2d(S.d_qd, S.h_d.p, per * nq, st);
+    S.h2d(S.d_qd, S.h_d.p, per * nq, st);
   }
 
   // ---- pairs and items ----
@@ -555,24 +541,21 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
         a_is[pair_item_start[p] + k] = chain_start[c] + k;
       }
     }
-    h2d(S.d_scan_pt_start, a_pt, nscans + 1, st);
-    h2d(S.d_pair_query, a_pq, npairs, st);
-    h2d(S.d_pair_chain, S.pair_chain.data(), npairs, st);
-    h2d(S.d_pair_item_start, a_pis, npairs + 1, st);
-    h2d(S.d_item_pair, a_ip, std::max(nitems, 1), st);
-    h2d(S.d_item_scan, a_is, std::max(nitems, 1), st);
+    S.h2d(S.d_scan_pt_start, a_pt, nscans + 1, st);
+    S.h2d(S.d_pair_query, a_pq, npairs, st);
+    S.h2d(S.d_pair_chain, S.pair_chain.data(), npairs, st);
+    S.h2d(S.d_pair_item_start, a_pis, npairs + 1, st);
+    S.h2d(S.d_item_pair, a_ip, std::max(nitems, 1), st);
+    S.h2d(S.d_item_scan, a_is, std::max(nitems, 1), st);
   }
   S.d_cells.reserve((size_t)std::max(nitems, 1) * S.max_n);
   S.d_cell_count.reserve(std::max(nitems, 1));
-  if (S.d_kernel.cap == 0) h2d(S.d_kernel, g0.kernel.data(), g0.kernel.size(), st);
+  if (S.d_kernel.cap == 0) S.h2d(S.d_kernel, g0.kernel.data(), g0.kernel.size(), st);
 
   // ---- workspaces: one per resident CTA ----
-  int dev = 0, sms = 132;
-  B200_CUDA(cudaGetDevice(&dev));
-  B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const size_t smem = (size_t)generic_slice_rows(nA, n) * n * sizeof(int32_t);
   const int per_sm = smem <= 100 * 1024 ? 2 : 1;
-  S.blocks = std::min(npairs, sms * per_sm);
+  S.blocks = std::min(npairs, h->sms * per_sm);
   const size_t gpitch = ((size_t)g0.data_size + 255) & ~(size_t)255;
   const size_t spitch = ((size_t)P * nA + 63) & ~(size_t)63;
   const size_t ppitch = ((size_t)5 * P + 31) & ~(size_t)31;
@@ -756,12 +739,6 @@ static bool finish_query_pair(const b200sm * h, SweepHost & S, int q, const Pair
   return true;
 }
 
-static bool finish_pair(const b200sm * h, SweepHost & S, int pair, const PairOut & o, double * response, double * mean, double * cov,
-                        int raster_empty = -1)
-{
-  return finish_query_pair(h, S, S.pair_query[pair], o, response, mean, cov, raster_empty);
-}
-
 static void chain_of_pair(const SweepHost & S, int pair, const b200_scan *& base, int & nbase)
 {
   int c = S.pair_chain[pair];
@@ -806,7 +783,7 @@ static int sweep_fetch(b200sm * h, bool do_refine, double * response, double * m
       if (!cell_count.empty())
         for (int it = item_start[p]; it < item_start[p + 1]; ++it) if (cell_count[it] > 0) { raster_empty = 0; break; }
     }
-    if (!finish_pair(h, S, p, S.h_out.p[p], &response[p], &mean[3 * p], &cov[9 * p], raster_empty)) {
+    if (!finish_query_pair(h, S, S.pair_query[p], S.h_out.p[p], &response[p], &mean[3 * p], &cov[9 * p], raster_empty)) {
       // tie-list overflow / response expansion: this pair goes through the single-match path
       const b200_scan * base; int nbase;
       chain_of_pair(S, p, base, nbase);
@@ -845,14 +822,9 @@ static int sweep_fetch(b200sm * h, bool do_refine, double * response, double * m
   const int n = S.n;
   const size_t no = (size_t)S.npairs * nA * n, np = (size_t)S.npairs * P, ns = (size_t)S.npairs * P * nA;
   S.h_i.reserve(no + np + ns);
-  for (int p = 0; p < S.npairs; ++p) {
-    for (size_t i = 0; i < (size_t)nA * n; ++i) S.h_i.p[(size_t)p * nA * n + i] = device_offset(fp[p].offsets[i], h->g.data_size);
-    for (int y = 0; y < fp[p].nY; ++y)
-      for (int x = 0; x < fp[p].nX; ++x)
-        S.h_i.p[no + (size_t)p * P + (size_t)y * fp[p].nX + x] = fp[p].xs[x] + fp[p].ys[y] * h->g.stride;
-  }
-  h2d(S.d_fine_off, S.h_i.p, no, st);
-  h2d(S.d_fine_pos, S.h_i.p + no, np, st);
+  for (int p = 0; p < S.npairs; ++p) device_plan(fp[p], h->g, S.h_i.p + (size_t)p * nA * n, S.h_i.p + no + (size_t)p * P);
+  S.h2d(S.d_fine_off, S.h_i.p, no, st);
+  S.h2d(S.d_fine_pos, S.h_i.p + no, np, st);
   S.d_fine_sums.reserve(ns);
   FineDev f{P, nA, S.d_fine_off.p, S.d_fine_pos.p, S.d_fine_sums.p};
   k_sweep_fine<<<S.blocks, kSweepThreads, 0, st>>>(S.dev, f);

@@ -960,6 +960,60 @@ void classify_beams(const GridGeom & g, const CorrPlan & pl, int a, int pitch_w,
   c.n_fast = nf; c.n_edge = ne;
 }
 
+void append_beam_lists(const std::vector<BeamClasses> & cls, int nstage, BeamLists & L)
+{
+  L.slow_start.push_back((int32_t)L.slow.size());
+  for (const BeamClasses & c : cls) {
+    L.slow.insert(L.slow.end(), c.far.begin(), c.far.end());
+    L.slow_start.push_back((int32_t)L.slow.size());
+    L.n_fast += c.n_fast; L.n_edge += c.n_edge;
+    for (int sg = 0; sg < nstage; ++sg) {
+      L.wrap2_start.push_back((int32_t)L.wrap2.size());
+      L.wrap2.insert(L.wrap2.end(), c.wrap2[sg].begin(), c.wrap2[sg].end());
+      for (int m = 0; m < 4; ++m) {
+        L.edge_start.push_back((int32_t)L.edge.size());
+        L.edge.insert(L.edge.end(), c.edge[sg * 4 + m].begin(), c.edge[sg * 4 + m].end());
+      }
+    }
+  }
+}
+
+void upload_beam_lists(BeamLists & L, SweepHost & S, cudaStream_t st)
+{
+  L.edge_start.push_back((int32_t)L.edge.size());
+  L.wrap2_start.push_back((int32_t)L.wrap2.size());
+  S.beam_counts[0] = L.n_fast; S.beam_counts[1] = L.n_edge; S.beam_counts[2] = (int32_t)L.slow.size();
+  L.edge.push_back(0); L.wrap2.push_back(0); L.slow.push_back(0);
+  S.h2d(S.d_edge, L.edge.data(), L.edge.size(), st);
+  S.h2d(S.d_edge_start, L.edge_start.data(), L.edge_start.size(), st);
+  S.h2d(S.d_wrap2, L.wrap2.data(), L.wrap2.size(), st);
+  S.h2d(S.d_wrap2_start, L.wrap2_start.data(), L.wrap2_start.size(), st);
+  S.h2d(S.d_slow, L.slow.data(), L.slow.size(), st);
+  S.h2d(S.d_slow_start, L.slow_start.data(), L.slow_start.size(), st);
+}
+
+void encode_runs(const std::vector<uint16_t> & group, int min_weight, bool merge, std::vector<uint16_t> & plain,
+                 std::vector<std::pair<uint16_t, uint16_t>> & merged)
+{
+  for (size_t i = 0; i < group.size();) {
+    size_t j = i;
+    while (j < group.size() && group[j] == group[i]) ++j;
+    if (merge && j - i >= (size_t)min_weight) merged.emplace_back(group[i], (uint16_t)(j - i));
+    else plain.insert(plain.end(), j - i, group[i]);
+    i = j;
+  }
+}
+
+int parity_refusal(const GridGeom & g, const std::vector<CorrPlan> & plans)
+{
+  if (g.order_dependent) return 1;   // AddScan's occupancy test makes the raster sequential (generic kernel)
+  for (const CorrPlan & pl : plans) {
+    for (int k = 1; k < pl.nX; ++k) if (pl.xs[k] != pl.xs[0] + 2 * k) return 6;
+    for (int k = 1; k < pl.nY; ++k) if (pl.ys[k] != pl.ys[0] + 2 * k) return 7;
+  }
+  return 0;
+}
+
 bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
 {
   const GridGeom & g = h->g;
@@ -986,13 +1040,8 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   //   item pb / pe (16 bits)       payload entries of one block                                -> 11
   //   TileSeq.off (int32)          descriptor blob bytes                                       -> 12
   //   cell-list staging            max_n > 4096: the raster reads the cells from global memory    (no refusal needed)
-  if (g.order_dependent) return bail(1);                // AddScan's occupancy test makes the raster sequential (generic kernel)
+  if (const int why = parity_refusal(g, S.plans)) return bail(why);
   if ((g.stride & 1) || nA < 1 || nA > 4096) return bail(2);
-  for (int q = 0; q < nq; ++q) {
-    const CorrPlan & pl = S.plans[q];
-    for (int k = 1; k < nX; ++k) if (pl.xs[k] != pl.xs[0] + 2 * k) return bail(6);   // coarse step must be exactly 2 cells
-    for (int k = 1; k < nY; ++k) if (pl.ys[k] != pl.ys[0] + 2 * k) return bail(7);
-  }
   // ---- geometry of one parity sub-grid ----
   int pitch_w = (g.stride / 2 + 16 + 3) / 4;             // sub-grid row + the 3-word overhang of the last x-tile
   while ((pitch_w & 7) != 4) ++pitch_w;                  // 8 rows x 4 words of a warp hit 32 distinct banks
@@ -1010,9 +1059,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   const int halo = nY + 2;                               // rows a beam window reaches below its base row (idle row tiles are clamped) + the wrapped row
   const int base_rows = std::max(1, rows_valid - nY + 1);   // distinct base rows of beams whose window is inside the grid
   // ---- choose the number of angle chunks V and of bands ----
-  int sms = 132, dev = 0;
-  B200_CUDA(cudaGetDevice(&dev));
-  B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int sms = h->sms;
   int want_c = h->tile_cluster > 0 ? h->tile_cluster : env_int("B200_SWEEP_CLUSTER", 0);
   if (want_c <= 0) {
     // throughput mode (one CTA per pair) once the batch fills the GPU, otherwise spread a pair over a cluster
@@ -1101,10 +1148,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   std::vector<uint8_t> blob;
   std::vector<TileSeq> seq;
   std::vector<int32_t> seq_start((size_t)nq * C + 1, 0);
-  std::vector<int32_t> edge, edge_start((size_t)nq * nA * nstage * 4 + 1, 0);
-  std::vector<int32_t> wrap2, wrap2_start((size_t)nq * nA * nstage + 1, 0);
-  std::vector<int32_t> slow, slow_start((size_t)nq * (nA + 1), 0);
-  int n_fast = 0, n_edge = 0;
+  BeamLists lists;
   std::vector<BeamClasses> cls(nA);
   blob.reserve((size_t)nq * nA * n * 2 + 4096);
   struct Encoded { int32_t tbl[16]; std::vector<uint16_t> pay; };
@@ -1128,26 +1172,18 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
           // run-length encode: beams that land in the same cell share one entry of weight k (one load per row, fields times
           // k), provided the whole group fits one flush.  Entries of equal weight are then paired (two loads added byte-wise,
           // one multiply per field); weight-1 beams stay in the plain list.
-          const bool dedup = !h->no_dedup && gk.size() <= (size_t)kChunkBeams;
-          std::vector<std::pair<uint16_t, uint16_t>> multi;   // (weight, offset)
-          for (size_t i = 0; i < gk.size();) {
-            size_t j = i;
-            while (j < gk.size() && gk[j] == gk[i]) ++j;
-            const size_t cnt = j - i;
-            if (dedup && cnt >= (pairs_on ? 2u : 3u)) multi.emplace_back((uint16_t)cnt, gk[i]);
-            else for (size_t t = 0; t < cnt; ++t) pay.push_back(gk[i]);
-            i = j;
-          }
+          std::vector<std::pair<uint16_t, uint16_t>> multi;   // (offset, weight), by ascending weight
+          encode_runs(gk, pairs_on ? 2 : 3, !h->no_dedup && gk.size() <= (size_t)kChunkBeams, pay, multi);
           std::stable_sort(multi.begin(), multi.end(),
-                           [](const std::pair<uint16_t, uint16_t> & x, const std::pair<uint16_t, uint16_t> & y) { return x.first < y.first; });
+                           [](const std::pair<uint16_t, uint16_t> & x, const std::pair<uint16_t, uint16_t> & y) { return x.second < y.second; });
           std::vector<std::pair<uint16_t, uint16_t>> single;   // (offset, weight)
           std::vector<uint16_t> pairs;                         // offset, offset, weight, 0
           for (size_t i = 0; i < multi.size();) {
-            if (pairs_on && i + 1 < multi.size() && multi[i + 1].first == multi[i].first) {
-              pairs.insert(pairs.end(), {multi[i].second, multi[i + 1].second, multi[i].first, (uint16_t)0});
+            if (pairs_on && i + 1 < multi.size() && multi[i + 1].second == multi[i].second) {
+              pairs.insert(pairs.end(), {multi[i].first, multi[i + 1].first, multi[i].second, (uint16_t)0});
               i += 2;
             } else {
-              single.emplace_back(multi[i].second, multi[i].first);
+              single.push_back(multi[i]);
               i += 1;
             }
           }
@@ -1179,23 +1215,7 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
       }
     };
     host_parallel_for(nA, one_angle);
-    for (int a = 0; a < nA; ++a) {
-      slow_start[(size_t)q * (nA + 1) + a] = (int32_t)slow.size();
-      slow.insert(slow.end(), cls[a].far.begin(), cls[a].far.end());
-      n_fast += cls[a].n_fast; n_edge += cls[a].n_edge;
-    }
-    slow_start[(size_t)q * (nA + 1) + nA] = (int32_t)slow.size();
-    for (int a = 0; a < nA; ++a)
-      for (int sg = 0; sg < nstage; ++sg) {
-        wrap2_start[((size_t)q * nA + a) * nstage + sg] = (int32_t)wrap2.size();
-        const auto & w = cls[a].wrap2[sg];
-        wrap2.insert(wrap2.end(), w.begin(), w.end());
-        for (int m = 0; m < 4; ++m) {
-          edge_start[(((size_t)q * nA + a) * nstage + sg) * 4 + m] = (int32_t)edge.size();
-          const auto & ev = cls[a].edge[sg * 4 + m];
-          edge.insert(edge.end(), ev.begin(), ev.end());
-        }
-      }
+    append_beam_lists(cls, nstage, lists);
     std::vector<uint16_t> pay;
     std::vector<int32_t> tbl;
     std::vector<int> nedge;
@@ -1269,21 +1289,13 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     }
   }
   seq_start[(size_t)nq * C] = (int32_t)seq.size();
-  edge_start[(size_t)nq * nA * nstage * 4] = (int32_t)edge.size();
-  wrap2_start[(size_t)nq * nA * nstage] = (int32_t)wrap2.size();
-  S.tile_stats[7] = (int32_t)wrap2.size();
-  edge.push_back(0); wrap2.push_back(0); slow.push_back(0);
+  S.tile_stats[7] = (int32_t)lists.wrap2.size();
   blob.resize(blob.size() + 16, 0);
 
-  h2d(S.d_tile_desc, blob.data(), blob.size(), st);
-  h2d(S.d_tile_seq, seq.data(), seq.size(), st);
-  h2d(S.d_tile_seq_start, seq_start.data(), seq_start.size(), st);
-  h2d(S.d_edge, edge.data(), edge.size(), st);
-  h2d(S.d_edge_start, edge_start.data(), edge_start.size(), st);
-  h2d(S.d_wrap2, wrap2.data(), wrap2.size(), st);
-  h2d(S.d_wrap2_start, wrap2_start.data(), wrap2_start.size(), st);
-  h2d(S.d_slow, slow.data(), slow.size(), st);
-  h2d(S.d_slow_start, slow_start.data(), slow_start.size(), st);
+  S.h2d(S.d_tile_desc, blob.data(), blob.size(), st);
+  S.h2d(S.d_tile_seq, seq.data(), seq.size(), st);
+  S.h2d(S.d_tile_seq_start, seq_start.data(), seq_start.size(), st);
+  upload_beam_lists(lists, S, st);
   T.desc = S.d_tile_desc.p; T.seq = S.d_tile_seq.p; T.seq_start = S.d_tile_seq_start.p;
   T.edge = S.d_edge.p; T.edge_start = S.d_edge_start.p;
   T.wrap2 = S.d_wrap2.p; T.wrap2_start = S.d_wrap2_start.p;
@@ -1313,7 +1325,6 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
   S.tile_info[0] = 1; S.tile_info[1] = C; S.tile_info[2] = V; S.tile_info[3] = nbands; S.tile_info[4] = B; S.tile_info[5] = 0;
   S.tile_info[6] = clusters; S.tile_info[7] = (int32_t)(smem / 1024);
   S.tile_layout[0] = ytile_rows; S.tile_layout[1] = ytiles; S.tile_layout[2] = xtiles; S.tile_layout[3] = tail ? 1 : 0;
-  S.beam_counts[0] = n_fast; S.beam_counts[1] = n_edge; S.beam_counts[2] = (int32_t)slow.size() - 1;
   return true;
 }
 

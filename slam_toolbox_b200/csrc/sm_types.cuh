@@ -14,6 +14,9 @@ namespace b200 {
 constexpr int kMaxTies = 24;          // tie indices returned per pair; more -> host re-runs the pair
 constexpr int kSweepThreads = 512;
 constexpr int32_t kDevInvalid = -(1 << 30);   // device lookup sentinel: pos + it is always < 0
+// shared memory a correlation kernel may fill with lookup rows (k_correlate: one row, k_sweep_generic: a slice of rows); a query
+// needs at least one row, so it may have at most 51,200 readings
+constexpr size_t kLookupSmemBytes = 200 * 1024;
 
 // CorrelationGrid geometry (M.h:1074-1313, K.h:4572-4965) + smear kernel
 struct GridGeom {
@@ -133,9 +136,9 @@ struct FastDev {
   const uint16_t * mult;         // multiplicity of every entry (1 for plain entries)
   const int32_t * cls_start;     // [nq][nA][33]: group g = phase * 4 + m -> [2g] plain begin, [2g+1] multi begin, [2g+2] end
   const int32_t * edge;          // EDGE beams in word form, grouped like the FAST lists: sub-row | word << 16 (both signed 16 bit)
-  const int32_t * edge_start;    // [nq][nA][17]
+  const int32_t * edge_start;    // CSR over ((q * nA + a) * 4 + phase) * 4 + m
   const int32_t * wrap2;         // EDGE beams whose columns leave [0, stride): secondary entries (row parity flipped)
-  const int32_t * wrap2_start;   // [nq][nA][4] + 1, per phase
+  const int32_t * wrap2_start;   // CSR over (q * nA + a) * 4 + phase
   const int32_t * slow;          // FAR beams (column offsets >= one stride): device-form linear offsets
   const int32_t * slow_start;    // [nq][nA + 1]
 };
@@ -215,7 +218,7 @@ struct SweepHost {
   std::vector<int32_t> chain_start;
   DevBuf<int32_t> d_offsets, d_posidx, d_scan_pt_start, d_pair_query, d_pair_chain, d_pair_item_start, d_item_pair, d_item_scan,
     d_cells, d_cell_count, d_ws_sums, d_fine_off, d_fine_pos, d_fine_sums;
-  DevBuf<double> d_qgeom, d_center, d_qd, d_angpen, d_points, d_ws_probs;
+  DevBuf<double> d_qd, d_points, d_ws_probs;
   DevBuf<uint8_t> d_ws_grid, d_kernel, d_win_flag;
   // the sweep kernel the upload chose (kSweepGeneric / kSweepFast / kSweepTile) and, when that is the generic kernel, why the
   // parity kernels were refused (b200sm_batch_info)
@@ -245,7 +248,7 @@ struct SweepHost {
   DevBuf<int32_t> d_tile_seq_start;
   DevBuf<PairOut> d_out;
   PinBuf<PairOut> h_out;
-  PinBuf<uint8_t> arena;    // pinned staging of the upload's tables (sweep_stage_h2d)
+  PinBuf<uint8_t> arena;    // pinned staging of the upload's tables (stage)
   size_t arena_used = 0;
   PinBuf<int32_t> h_i;
   PinBuf<double> h_d;
@@ -257,6 +260,15 @@ struct SweepHost {
   double upload_ms[3] = {0, 0, 0};   // host wall time of the last upload: lookup tables (plans), kernel tables, whole call
   ZeroCache zero, zero_exp;   // all-poses-tie results per query: of the coarse pass, of the widest response-expansion pass
   void release();
+  // bytes host -> device through the arena, counted in h2d_bytes
+  void stage(void * dst, const void * src, size_t bytes, cudaStream_t s);
+  // count elements into dst (grown as needed) through the arena
+  template <class T>
+  void h2d(DevBuf<T> & dst, const T * src, size_t count, cudaStream_t s)
+  {
+    dst.reserve(count);
+    stage(dst.p, src, count * sizeof(T), s);
+  }
 };
 
 }  // namespace b200
@@ -270,6 +282,7 @@ struct b200sm {
   int64_t launches = 0;
   double phase_ms[6] = {0, 0, 0, 0, 0, 0};   // host-side phase times of the single-match path (b200sm_match_timing)
   int probs_side = 0;   // Grid<double> m_pSearchSpaceProbs side (M.cpp:513)
+  int sms = 132;        // multiprocessor count of the device the handle was created on
 
   // single-match device state
   b200::DevBuf<uint8_t> d_grid, d_kernel;
@@ -300,6 +313,8 @@ namespace b200 {
 double do_match(b200sm * h, const b200_scan * query, const b200_scan * base, int nbase, bool pen, bool refine,
                 double mean[3], double cov[9]);
 int32_t device_offset(int32_t off, int data_size);
+// device form of a plan: its nA x n lookup rows to offsets (device_offset), the grid index of every pose to posidx [nY][nX]
+void device_plan(const CorrPlan & pl, const GridGeom & g, int32_t * offsets, int32_t * posidx);
 void set_grid_offset(GridGeom & g, const b200_scan * query);
 double normalize_angle_difference(double minuend, double subtrahend);
 }  // namespace b200
@@ -323,21 +338,31 @@ struct BeamClasses {
 // pitch_w = sub-grid row pitch in words; nbands bands of band_rows sub-rows each, the last one open-ended
 void classify_beams(const GridGeom & g, const CorrPlan & pl, int a, int pitch_w, int band_rows, int nbands, BeamClasses & c);
 
+// The EDGE / wrap2 / FAR lists of the parity kernel that runs, over all queries of a sweep: edge_start is a CSR over
+// ((q * nA + a) * nstage + stage) * 4 + m, wrap2_start one over (q * nA + a) * nstage + stage (nstage = 4 * nbands), slow_start
+// [nq][nA + 1] indexes slow.  n_fast / n_edge count the FAST beams and the EDGE beams with a primary entry.
+struct BeamLists {
+  std::vector<int32_t> edge, edge_start, wrap2, wrap2_start, slow, slow_start;
+  int32_t n_fast = 0, n_edge = 0;
+};
+// appends one query's classes (cls[a] for every angle a, nstage stages each)
+void append_beam_lists(const std::vector<BeamClasses> & cls, int nstage, BeamLists & L);
+// terminates the lists, copies them to S.d_edge .. S.d_slow_start and sets S.beam_counts to the FAST, EDGE and FAR beams
+void upload_beam_lists(BeamLists & L, SweepHost & S, cudaStream_t st);
+// Run-length encoding of one sorted FAST group: a run of at least min_weight beams on one cell becomes one merged (offset,
+// weight) entry when merge is set, every other beam one plain entry.  Appends both kinds in offset order.
+void encode_runs(const std::vector<uint16_t> & group, int min_weight, bool merge, std::vector<uint16_t> & plain,
+                 std::vector<std::pair<uint16_t, uint16_t>> & merged);
+// The refusal code of the preconditions both parity kernels share, 0 when they hold: an order-independent raster (1) and coarse
+// steps of exactly 2 cells in x (6) and y (7) in every plan.
+int parity_refusal(const GridGeom & g, const std::vector<CorrPlan> & plans);
+
 // The builders of the parity kernels' tables return false, with a refusal code in fast_refusal / tile_info[5], when their kernel
 // cannot run the uploaded sweep.  They copy nothing to the device before their last refusal.
 bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st);
 bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st);
 void launch_sweep_fast(SweepHost & S, cudaStream_t st);
 void launch_sweep_tile(SweepHost & S, cudaStream_t st);
-
-void sweep_stage_h2d(void * dst, const void * src, size_t bytes, cudaStream_t s);
-// count elements into dst (grown as needed) through the upload's pinned staging arena (sweep_stage_h2d)
-template <class T>
-inline void h2d(DevBuf<T> & dst, const T * src, size_t count, cudaStream_t s)
-{
-  dst.reserve(count);
-  sweep_stage_h2d(dst.p, src, count * sizeof(T), s);
-}
 
 // ScanMatcher::CorrelateScan's reduction + covariance (M.cpp:775-1025) on the host from an integer volume
 double host_epilogue(const b200sm_params & prm, const GridGeom & geom, int probs_side, const CorrPlan & pl,
