@@ -135,9 +135,9 @@ def poses_near(world: World, center_xy, radius: float, n: int, rng: np.random.Ge
 
 
 def noisy(ranges: np.ndarray, rng: np.random.Generator, sigma: float = 0.01, inf_frac: float = 0.0,
-          nan_frac: float = 0.0) -> np.ndarray:
+          nan_frac: float = 0.0, range_max: float = RANGE_MAX) -> np.ndarray:
     r = ranges + rng.normal(0.0, sigma, ranges.shape)
-    r = np.clip(r, 0.0, RANGE_MAX)
+    r = np.clip(r, 0.0, range_max)
     if inf_frac > 0:
         r = np.where(rng.random(r.shape) < inf_frac, np.inf, r)
     if nan_frac > 0:
@@ -670,6 +670,36 @@ def make_highres_sweep(n_beams: int, fov_deg: float, *, seed: int = 11, n_querie
     cr = noisy(raycast(world, cposes, n_beams=n_beams, angle_min=amin, angle_inc=inc), rng, inf_frac=inf_frac)
     chain_start = np.arange(0, n_chains * chain_len + 1, chain_len, dtype=np.int32)
     return AdversarialSweep(qr, qpose, cr, cposes, chain_start, (amin, inc), (amin, inc))
+
+
+def make_long_range_sweep(range_threshold: float, *, beyond: bool = False, seed: int = 17, n_queries: int = 1,
+                          n_chains: int = 2, radius: float = 3.0) -> AdversarialSweep:
+    """Room scans of the standard 1081-beam laser for a matcher whose range threshold is range_threshold (rt) metres, in a
+    world scaled to the range: make_world(seed, 6 rt, 1.5 rt, 3 rt), rooms 1.5 to 3 rt across (at rt = 40 m: 240 m, rooms of
+    60 to 120 m).  The queries look along +x, so that the laser's 270 deg field of view covers both +y and -y; with the default
+    seed the first query sees past rt in both.
+
+    beyond=False clips the readings at rt (a lidar whose range_max is the threshold): the query's beams reach the correlation
+    grid's first and last row bands and stay inside the grid.  beyond=True lets the lidar see 5 rt, like a long-range lidar
+    under a shorter max_laser_range: the matcher takes the unfiltered readings, so the readings past rt are query beams whose
+    pose window leaves the grid (EDGE and row-wrapped beams).  The room walls hide everything past about 3 rt, so every 8th
+    query reading within 20 deg of the heading reads 5 rt instead (a distant structure): those beams' columns leave the grid by
+    more than its width (FAR beams).  Queries get make_loop_sweep's drift; candidate chains start within `radius` of the first
+    query."""
+    rng = np.random.default_rng(seed)
+    k = range_threshold / 40.0
+    world = make_world(seed, size=240.0 * k, min_room=60.0 * k, max_room=120.0 * k)
+    lidar = 5.0 * range_threshold if beyond else range_threshold
+    qtrue = np.array([free_pose(world, rng, margin=2.0) for _ in range(n_queries)])
+    qtrue[:, 2] = 0.0
+    qr = noisy(raycast(world, qtrue, range_max=lidar), rng, range_max=lidar)
+    if beyond:
+        ahead = np.flatnonzero(np.abs(ANGLE_MIN + np.arange(N_BEAMS) * ANGLE_INC) <= math.radians(20.0))
+        qr[:, ahead[::8]] = lidar
+    qpose = qtrue + np.column_stack([rng.normal(0, 0.5, (n_queries, 2)), rng.normal(0, 0.08, n_queries)])
+    cposes = poses_near(world, qtrue[0, :2], radius, n_chains, rng)
+    cr = noisy(raycast(world, cposes, range_max=lidar), rng, range_max=lidar)
+    return AdversarialSweep(qr, qpose, cr, cposes, np.arange(n_chains + 1, dtype=np.int32))
 
 
 WEIGHTED_BEAMS = 8192   # laser of make_weighted_sweep: 360 deg at 0.044 deg

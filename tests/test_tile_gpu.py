@@ -165,26 +165,40 @@ def test_empty_chains_and_ragged_chain_lengths():
 
 def test_other_search_windows_and_angle_resolutions():
     """Geometries away from the shipped ones: 41 angles (1 degree steps), a 3 m window at a 10 m range threshold (run-time row pitch
-    instantiation), a 0.1 m grid, and a 5 x 5 smear kernel with six distinct values (CAS raster) -- auto plan and 2-CTA clusters."""
+    instantiation), a 0.1 m grid, and a 5 x 5 smear kernel with six distinct values (CAS raster) -- auto plan and 2-CTA clusters.
+    Wide smear kernels at 0.05 m cells: 15 x 15 taps (sigma 0.18 m, the last kernel held in TileShared::kern), 17 x 17 (0.19 m,
+    read from global memory) and 41 x 41 (0.499 m, the widest order-independent kernel); at sigma 0.4995 m the taps next to the
+    centre round to 100, the raster is order dependent and the sweep runs on the generic kernel (refusal 100 + 1)."""
     import math
-    cases = [
-        (dict(H.MAPPER_LOOP, coarse_angle_resolution=math.radians(1.0), use_response_expansion=0), (3.0, 0.05, 0.03, 10.0)),
-        (dict(H.MAPPER_LOOP, coarse_search_angle_offset=math.radians(10.0), use_response_expansion=0), (6.0, 0.1, 0.1, 15.0)),
-        (dict(H.MAPPER_LOOP, use_response_expansion=0), (5.0, 0.05, 0.05, 14.0)),
-        (dict(H.MAPPER_LOOP, use_response_expansion=0), H.GRID_SMALL),                      # 6 x 6 poses: tiny accumulators
-        (dict(H.MAPPER_LOOP, use_response_expansion=0), (0.5, 0.05, 0.03, 20.0)),           # ... behind a wide row pitch
+    loop = dict(H.MAPPER_LOOP, use_response_expansion=0)
+    cases = [   # (mapper, grid, smear kernel size or None, refusal of the tiled planner)
+        (dict(H.MAPPER_LOOP, coarse_angle_resolution=math.radians(1.0), use_response_expansion=0), (3.0, 0.05, 0.03, 10.0), None, 0),
+        (dict(H.MAPPER_LOOP, coarse_search_angle_offset=math.radians(10.0), use_response_expansion=0), (6.0, 0.1, 0.1, 15.0), None, 0),
+        (loop, (5.0, 0.05, 0.05, 14.0), None, 0),
+        (loop, H.GRID_SMALL, None, 0),                      # 6 x 6 poses: tiny accumulators
+        (loop, (0.5, 0.05, 0.03, 20.0), None, 0),           # ... behind a wide row pitch
+        (loop, (4.0, 0.05, 0.18, 12.0), 15, 0),
+        (loop, (4.0, 0.05, 0.19, 12.0), 17, 0),
+        (loop, (4.0, 0.05, 0.499, 12.0), 41, 0),
+        (loop, (4.0, 0.05, 0.4995, 12.0), 41, 1),
     ]
     sw = synth.make_loop_sweep(81, n_queries=1, n_chains=5, chain_len=2, inf_frac=0.02)
-    for mapper, grid in cases:
+    for mapper, grid, ksize, refusal in cases:
         pm, gm = H.port_matcher(mapper, grid), H.gpu_matcher(mapper, grid)
+        if ksize:
+            assert pm.grid()["kernel_size"] == ksize, grid
         gc, gq = H.gpu_block(sw.cand_ranges, sw.cand_poses), H.gpu_block(sw.query_ranges, sw.query_poses)
         er, em, ec = _expected(pm, sw, 1, 5)
         for cluster in (0, 1, 2):
             gm.set_option("sweep_cluster", cluster)
             r, m, c, _ = _run(gm, gq, gc, sw)
-            info = gm.batch_info()
-            assert info["kernel"] == "tile", (grid, info)
-            assert np.array_equal(r, er) and np.array_equal(m, em) and np.array_equal(c, ec), (grid, cluster, gm.batch_tile_info())
+            info, plan = gm.batch_info(), gm.batch_tile_info()
+            if refusal:
+                assert info["kernel"] == "generic" and info["refused_reason"] == 100 + refusal, (grid, info)
+                assert plan["refused_reason"] == refusal, (grid, plan)
+            else:
+                assert info["kernel"] == "tile", (grid, info)
+            assert np.array_equal(r, er) and np.array_equal(m, em) and np.array_equal(c, ec), (grid, cluster, plan)
 
 
 def test_plan_readouts_describe_the_last_upload():
