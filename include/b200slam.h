@@ -332,6 +332,9 @@ int b200pg_factor_info(const b200pg * h, int64_t info[8]);
 #define B200_CELL_OCCUPIED 100   /* GridStates_Occupied Karto.h:4380 */
 #define B200_CELL_FREE 255       /* GridStates_Free     Karto.h:4381 */
 
+/* The three laser fields are the DEFAULT limits: those of every scan added by b200og_add_scans (or with a NULL laser
+ * array).  A scan added by b200og_add_scans_lasers carries its own limits, as the reference reads each scan's own
+ * pScan->GetLaserRangeFinder() (Karto.h:6146-6151, :5646-5698). */
 typedef struct b200og_params {
   double resolution;           /* m per cell (CreateFromScans' argument); 0 is rejected (Karto.h:5916-5918) */
   double range_threshold;      /* LaserRangeFinder::GetRangeThreshold(): longer readings are traced up to it, without a hit */
@@ -357,6 +360,15 @@ int b200og_set_stream(b200og * h, void * cuda_stream);
 /* The scan store.  add = copy n scans (ranges, unfiltered point readings, sensor position) to the
  * device, after the scans already there; clear = forget them all. */
 int b200og_add_scans(b200og * h, const b200_scan * scans, int32_t n);
+/* One scan's laser limits, the values of its karto::LaserRangeFinder (see b200og_params). */
+typedef struct b200og_laser {
+  double range_threshold, minimum_range, maximum_range;
+} b200og_laser;
+/* b200og_add_scans with per-scan limits: lasers[i] belongs to scans[i] and is stored with it (24 B per scan on the
+ * device); builds, range builds, stored boxes and removals use each scan's own limits, so one store may hold the scans of
+ * several lasers.  lasers == NULL = the handle's params for every scan (b200og_add_scans is this call with NULL).
+ * B200_ERR_INVALID_ARG, with the store unchanged, for a non-finite limit. */
+int b200og_add_scans_lasers(b200og * h, const b200_scan * scans, int32_t n, const b200og_laser * lasers);
 int b200og_clear_scans(b200og * h);
 int32_t b200og_num_scans(const b200og * h);
 /* CreateFromScans over the stored scans.  With no scans the reference returns NULL: here

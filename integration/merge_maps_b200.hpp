@@ -14,6 +14,8 @@
 // so no tf2 type appears here).  The grids equal the reference's bit for bit: width, height, offset, cell bytes.  The
 // corrected scans stay on the device, so the karto scans the tool keeps are not corrected by this path; the sensor
 // position takes the points' formula, which is exact for a laser at the robot origin (GetSensorPose adds a zero offset).
+// Every scan is stored with its own laser's limits (each pose-graph file the tool loads brings its own laser), as the
+// reference's CreateFromScans reads them per scan.
 #pragma once
 #include <cstdio>
 #include <vector>
@@ -38,9 +40,12 @@ public:
   {
     if (grid) *grid = NULL;
     std::vector<b200_scan> scans;
+    std::vector<b200og_laser> lasers;
     for (LocalizedRangeScan * s : rScans) {
       if (s == nullptr) continue;                                   // Karto.h:6094, :6123
-      if (!laser_) laser_ = s->GetLaserRangeFinder();
+      LaserRangeFinder * l = s->GetLaserRangeFinder();
+      if (!laser_) laser_ = l;
+      lasers.push_back(b200og_laser{l->GetRangeThreshold(), l->GetMinimumRange(), l->GetMaximumRange()});
       b200_scan o;
       const PointVectorDouble & pts = s->GetPointReadings(false);
       o.n = static_cast<int32_t>(pts.size());
@@ -52,7 +57,7 @@ public:
     }
     if (!Ensure()) return -1;
     const int32_t first = b200og_num_scans(h_);
-    if (b200og_add_scans(h_, scans.data(), static_cast<int32_t>(scans.size())) != B200_OK) return Fail();
+    if (b200og_add_scans_lasers(h_, scans.data(), static_cast<int32_t>(scans.size()), lasers.data()) != B200_OK) return Fail();
     submaps_.push_back({first, static_cast<int32_t>(scans.size())});
     if (grid && !scans.empty()) *grid = Build(first, static_cast<int32_t>(scans.size()));
     return static_cast<int>(submaps_.size()) - 1;
@@ -130,7 +135,7 @@ private:
 
   kt_double resolution_;
   b200og * h_ = nullptr;
-  LaserRangeFinder * laser_ = nullptr;
+  LaserRangeFinder * laser_ = nullptr;   // the first scan's: the handle's default limits only
   std::vector<Range> submaps_;
 };
 

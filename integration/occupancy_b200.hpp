@@ -12,10 +12,17 @@
 // visualization_utils.hpp:108-146; map_saver; RayCast / IsFree).  The hit / pass counter grids inside it
 // stay empty: they are scratch of the CPU build (fetch them with b200og_fetch when wanted).
 //
+// Every scan is stored with its own laser's limits (scan->GetLaserRangeFinder(): range threshold, minimum and maximum
+// range), as the reference's AddScan and LocalizedRangeScan::Update read them (Karto.h:6146-6151, :5646-5698), so a map of
+// several lasers equals the reference's.
+//
 // ResidentOccupancyMap is the same publish with the scans kept on the device between calls (section 3a).
 #pragma once
 #include <cstdio>
 #include <cstring>
+#include <map>
+#include <set>
+#include <string>
 #include <vector>
 
 #include "karto_sdk/Karto.h"
@@ -26,14 +33,29 @@ namespace b200 {
 
 namespace detail {
 
-// the non-NULL scans of rScans as the C ABI takes them (pointers into the scans), and the laser of the first one
-inline std::vector<b200_scan> CollectScans(const LocalizedRangeScanVector & rScans, LaserRangeFinder ** laser)
+// a laser's limits as the store keeps them
+inline b200og_laser Limits(const LaserRangeFinder * l)
+{
+  return b200og_laser{l->GetRangeThreshold(), l->GetMinimumRange(), l->GetMaximumRange()};
+}
+
+inline bool SameLimits(const b200og_laser & a, const b200og_laser & b)
+{
+  return a.range_threshold == b.range_threshold && a.minimum_range == b.minimum_range && a.maximum_range == b.maximum_range;
+}
+
+// the non-NULL scans of rScans as the C ABI takes them (pointers into the scans), each scan's own laser limits
+// (GetLaserRangeFinder looks the laser up by the scan's sensor name, Karto.h:5304-5306), and the laser of the first one
+inline std::vector<b200_scan> CollectScans(const LocalizedRangeScanVector & rScans, std::vector<b200og_laser> * lasers,
+                                           LaserRangeFinder ** laser)
 {
   std::vector<b200_scan> scans;
   static_assert(sizeof(Vector2<kt_double>) == 2 * sizeof(double), "Vector2<double> must be {x, y}");
   for (LocalizedRangeScan * s : rScans) {
     if (s == nullptr) continue;                                   // Karto.h:6094, :6123
-    if (laser && !*laser) *laser = s->GetLaserRangeFinder();
+    LaserRangeFinder * l = s->GetLaserRangeFinder();
+    if (laser && !*laser) *laser = l;
+    if (lasers) lasers->push_back(Limits(l));
     b200_scan o;
     const PointVectorDouble & pts = s->GetPointReadings(false);  // Karto.h:6149
     o.n = static_cast<int32_t>(pts.size());
@@ -77,13 +99,17 @@ inline OccupancyGrid * CreateOccupancyGridFromScans(const LocalizedRangeScanVect
                                                      float * device_ms = nullptr)
 {
   LaserRangeFinder * laser = nullptr;
-  const std::vector<b200_scan> scans = detail::CollectScans(rScans, &laser);
+  std::vector<b200og_laser> lasers;
+  const std::vector<b200_scan> scans = detail::CollectScans(rScans, &lasers, &laser);
   if (rScans.empty()) return NULL;                                // Karto.h:5950-5952
   const b200og_params p = detail::GridParams(resolution, laser);
   b200og * h = nullptr;
   b200og_info info;
-  if (b200og_create_from_scans(&p, scans.data(), static_cast<int32_t>(scans.size()), &info, &h) != B200_OK) {
+  if (b200og_create(&p, &h) != B200_OK ||
+      b200og_add_scans_lasers(h, scans.data(), static_cast<int32_t>(scans.size()), lasers.data()) != B200_OK ||
+      b200og_build(h, &info) != B200_OK) {
     std::fprintf(stderr, "OccupancyGrid::CreateFromScans (b200): %s\n", b200_last_error());
+    b200og_destroy(h);
     return NULL;
   }
   OccupancyGrid * g = detail::FetchGrid(h, info, resolution);
@@ -92,14 +118,19 @@ inline OccupancyGrid * CreateOccupancyGridFromScans(const LocalizedRangeScanVect
   return g;
 }
 
-// The map publish with the scans resident on the device between publishes.  The store holds the scans of the last publish in
-// the order GetAllProcessedScans returned them (unique-id order).  A publish
+// The map publish with the scans resident on the device between publishes.  The store holds the scans of the last publish,
+// matched to the mapper's by unique id, in the order they were uploaded.  That need not be rScans' order (with several lasers
+// GetAllProcessedScans returns them sensor by sensor), and need not be: the grid does not depend on the scans' order (the
+// counters are integer sums, the box a min / max).  A publish
 //   - removes, in place (b200og_remove_scans), the stored scans the mapper no longer holds, such as the localization rolling
 //     buffer's oldest scans;
-//   - appends the scans whose unique ids are larger than every stored one (unique ids only grow);
+//   - appends the scans whose unique ids are not stored;
 //   - reloads every scan when poses_corrected is set, i.e. when MapperGraph::CorrectPoses has run since the last publish
 //     (b200_shim_correct_poses_calls() of integration/scan_matcher_b200.cpp counts its calls), since that moves stored scans'
-//     points, and whenever the scans are not in increasing unique-id order.
+//     points;
+//   - reloads every scan when the limits of a laser with stored scans changed since they were uploaded: the reference reads
+//     the laser's limits on every CreateFromScans, and every stored scan holds the limits of its upload.
+// The store is keyed on the resolution only: scans of any number of lasers share it, each with its own laser's limits.
 // The grid equals CreateOccupancyGridFromScans over the same scans.  One instance per map; not thread-safe.
 class ResidentOccupancyMap {
  public:
@@ -118,32 +149,43 @@ class ResidentOccupancyMap {
     for (LocalizedRangeScan * s : rScans)
       if (s) live.push_back(s);
     if (rScans.empty()) { if (stats) *stats = st; return NULL; }  // Karto.h:5950-5952
-    // the grid parameters as CreateOccupancyGridFromScans takes them on every call: the resolution and the first scan's laser
-    // limits.  The store is built for one set; another set starts a fresh store.
-    const b200og_params p = detail::GridParams(resolution, live.empty() ? nullptr : live[0]->GetLaserRangeFinder());
-    if (!h_ || !SameParams(p, params_)) {
+    // the store is built for one resolution; another one starts a fresh store.  The handle's own limits are never used: every
+    // scan is added with its laser's limits.
+    if (!h_ || resolution != resolution_) {
       if (h_) b200og_destroy(h_);
       h_ = nullptr;
       ids_.clear();
+      uploaded_.clear();
+      const b200og_params p = detail::GridParams(resolution, nullptr);
       if (b200og_create(&p, &h_) != B200_OK) return Fail();
-      params_ = p;
+      resolution_ = resolution;
       poses_corrected = true;
     }
-    bool increasing = true;
-    for (size_t k = 1; k < live.size() && increasing; ++k) increasing = live[k - 1]->GetUniqueId() < live[k]->GetUniqueId();
-    // stored scans that are gone, and where the new ones start
+    // the limits every laser of the live scans has now; a stored sensor whose limits changed since its upload reloads the store
+    std::map<std::string, b200og_laser> now;
+    for (LocalizedRangeScan * s : live) {
+      const std::string name = s->GetSensorName().ToString();
+      if (now.count(name)) continue;
+      now[name] = detail::Limits(s->GetLaserRangeFinder());
+    }
+    bool limits_changed = false;
+    for (const auto & kv : uploaded_) {
+      auto it = now.find(kv.first);
+      if (it != now.end() && !detail::SameLimits(it->second, kv.second)) limits_changed = true;
+    }
+    // stored scans that are gone, and the ones that stay
+    std::set<kt_int32s> live_ids, kept_ids;
+    for (LocalizedRangeScan * s : live) live_ids.insert(s->GetUniqueId());
     std::vector<int32_t> gone;
-    size_t next = 0;
-    bool reload = poses_corrected || !increasing;
+    const bool reload = poses_corrected || limits_changed;
     for (size_t k = 0; k < ids_.size() && !reload; ++k) {
-      if (next < live.size() && live[next]->GetUniqueId() == ids_[k]) { ++next; continue; }
-      if (next < live.size() && live[next]->GetUniqueId() < ids_[k]) reload = true;   // a scan older than a stored one is new
+      if (live_ids.count(ids_[k])) kept_ids.insert(ids_[k]);
       else gone.push_back(static_cast<int32_t>(k));
     }
     if (reload) {
       if (b200og_clear_scans(h_) != B200_OK) return Fail();
       ids_.clear();
-      next = 0;
+      uploaded_.clear();
       st.reloaded = 1;
     } else if (!gone.empty()) {
       if (b200og_remove_scans(h_, gone.data(), static_cast<int32_t>(gone.size())) != B200_OK) return Fail();
@@ -156,10 +198,18 @@ class ResidentOccupancyMap {
       ids_.swap(kept);
       st.removed = static_cast<int32_t>(gone.size());
     }
-    const LocalizedRangeScanVector added(live.begin() + next, live.end());
-    const std::vector<b200_scan> scans = detail::CollectScans(added, nullptr);
-    if (!scans.empty() && b200og_add_scans(h_, scans.data(), static_cast<int32_t>(scans.size())) != B200_OK) return Fail();
-    for (LocalizedRangeScan * s : added) ids_.push_back(s->GetUniqueId());
+    LocalizedRangeScanVector added;
+    for (LocalizedRangeScan * s : live)
+      if (!kept_ids.count(s->GetUniqueId())) added.push_back(s);
+    std::vector<b200og_laser> lasers;
+    const std::vector<b200_scan> scans = detail::CollectScans(added, &lasers, nullptr);
+    if (!scans.empty() && b200og_add_scans_lasers(h_, scans.data(), static_cast<int32_t>(scans.size()), lasers.data()) != B200_OK)
+      return Fail();
+    for (LocalizedRangeScan * s : added) {
+      ids_.push_back(s->GetUniqueId());
+      const std::string name = s->GetSensorName().ToString();
+      uploaded_[name] = now[name];
+    }
     st.appended = static_cast<int32_t>(scans.size());
     if (stats) *stats = st;
     b200og_info info;
@@ -169,13 +219,6 @@ class ResidentOccupancyMap {
   }
 
  private:
-  static bool SameParams(const b200og_params & a, const b200og_params & b)
-  {
-    return a.resolution == b.resolution && a.range_threshold == b.range_threshold && a.minimum_range == b.minimum_range &&
-           a.maximum_range == b.maximum_range && a.min_pass_through == b.min_pass_through &&
-           a.occupancy_threshold == b.occupancy_threshold;
-  }
-
   // after a failed call the store's contents are unknown: the next publish starts from a fresh handle
   OccupancyGrid * Fail()
   {
@@ -183,12 +226,14 @@ class ResidentOccupancyMap {
     if (h_) b200og_destroy(h_);
     h_ = nullptr;
     ids_.clear();
+    uploaded_.clear();
     return NULL;
   }
 
   b200og * h_ = nullptr;
-  b200og_params params_{};       // what h_ was created with
-  std::vector<kt_int32s> ids_;   // unique ids of the stored scans, in store order
+  kt_double resolution_ = 0.0;                   // what h_ was created with
+  std::vector<kt_int32s> ids_;                   // unique ids of the stored scans, in store order
+  std::map<std::string, b200og_laser> uploaded_;   // sensor name -> the limits its stored scans were uploaded with
 };
 
 }  // namespace b200

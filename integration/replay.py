@@ -11,6 +11,7 @@ Each run happens in its own process (both libraries define the same karto symbol
 from __future__ import annotations
 
 import ctypes as C
+import json
 import math
 import os
 import subprocess
@@ -71,7 +72,20 @@ def _bind(which: str):
     L.krep_occupancy_resident.argtypes = [C.c_void_p, C.c_double, C.POINTER(C.c_int), _DP, C.POINTER(C.c_uint8), C.c_long,
                                           C.POINTER(C.c_int), C.POINTER(C.c_float)]
     L.krep_init_laser.argtypes = [C.c_double] * 6
+    L.krep_laser.argtypes = [C.c_char_p] + [C.c_double] * 6
+    L.krep_process_on.argtypes = [C.c_void_p, C.c_char_p, _DP, C.c_int, _DP, C.c_int]
     return L
+
+
+SECOND_LASER = "laser1"
+
+
+def _second_laser(L, laser: dict):
+    """registers (or sets the limits of) the second laser, SECOND_LASER"""
+    n = L.krep_laser(SECOND_LASER.encode(), laser["min_angle"], laser["max_angle"], laser["ang_res"], laser["min_range"],
+                     laser["max_range"], laser["range_threshold"])
+    if n <= 0:
+        raise RuntimeError("krep_laser refused the second laser")
 
 
 def _create(L, laser: dict, params: dict, use_solver: bool):
@@ -186,16 +200,29 @@ def _publish_pair(L, h, map_resolution: float, step: int, log: list):
 
 
 def run_inprocess(which: str, ranges: np.ndarray, odom: np.ndarray, params: dict, laser: dict, use_solver: bool = True,
-                  map_resolution: float = 0.0, publish_every: int = 0, events=()):
+                  map_resolution: float = 0.0, publish_every: int = 0, events=(), sensors=None, laser2=None, laser2_changes=()):
     L = _bind(which)
     h = _create(L, laser, params, use_solver)
+    if laser2 is not None:
+        _second_laser(L, laser2)
     ranges = np.ascontiguousarray(ranges, dtype=np.float64)
     odom = np.ascontiguousarray(odom, dtype=np.float64)
     kept, publishes, removals = [], [], []
     buffer = int(params.get("scan_buffer_size", YAML_PARAMS["scan_buffer_size"]))
     for i in range(len(ranges)):
-        if L.krep_process(h, ranges[i].ctypes.data_as(_DP), ranges.shape[1], odom[i].ctypes.data_as(_DP), i):
+        if sensors is not None and sensors[i]:
+            done = L.krep_process_on(h, SECOND_LASER.encode(), ranges[i].ctypes.data_as(_DP), ranges.shape[1],
+                                     odom[i].ctypes.data_as(_DP), i)
+        else:
+            done = L.krep_process(h, ranges[i].ctypes.data_as(_DP), ranges.shape[1], odom[i].ctypes.data_as(_DP), i)
+        if done:
             kept.append(i)
+        for step, lim in laser2_changes:
+            if step == i:   # a publish with the store current, the change, then two publishes with no scan in between
+                _publish_pair(L, h, map_resolution, i, publishes)
+                _second_laser(L, dict(laser2, **lim))
+                _publish_pair(L, h, map_resolution, i, publishes)
+                _publish_pair(L, h, map_resolution, i, publishes)
         if publish_every and (i + 1) % publish_every == 0:
             _publish_pair(L, h, map_resolution, i, publishes)
         for ev in events:
@@ -218,7 +245,7 @@ def run_inprocess(which: str, ranges: np.ndarray, odom: np.ndarray, params: dict
                process_seconds=st[0], solver_computes=int(st[1]), solver_ms=st[2], edges=int(st[3]), scans=int(st[4]), match_calls=matches)
     if map_resolution:
         _occupancy(L, h, map_resolution, out)
-    if publish_every or events:
+    if publish_every or events or laser2_changes:
         out["publishes"] = np.array(publishes, dtype=np.float64).reshape(-1, 8)
     if events:
         out["removals"] = np.array(removals, dtype=np.int64).reshape(-1, 11)
@@ -228,12 +255,16 @@ def run_inprocess(which: str, ranges: np.ndarray, odom: np.ndarray, params: dict
 
 
 def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpdir=None, map_resolution=0.0, publish_every=0,
-        events=()):
+        events=(), sensors=None, laser2=None, laser2_changes=()):
     """Runs the replay in a fresh process and returns its result dict.  publish_every = k > 0 (with map_resolution) also
     publishes the map after every k-th scan through the resident store and the reference, 'publishes' rows as _publish_pair.
     events: after step i's scan, in list order, (i, "remove_node", id) removes a scan as lifelong mode does (krep_remove_node;
     id < 0 picks one of lifelong_candidates, see _remove_node; 'removals' rows) and (i, "publish") publishes as
-    publish_every does.  With events the result also holds the mapper's final edges and scan ids."""
+    publish_every does.  With events the result also holds the mapper's final edges and scan ids.
+    Two lasers: laser2 (a dict like laser, same angles) is registered as SECOND_LASER, and scan i is processed on it where
+    sensors[i] is nonzero (krep_process_on), on the first laser elsewhere.  laser2_changes = [(i, {key: value})] sets those
+    limits of the second laser after step i's scan: one publish before the change, then two after it with no scan in between
+    ('publishes' rows with step i)."""
     import tempfile
     params = params or YAML_PARAMS
     laser = laser or DEFAULT_LASER
@@ -242,7 +273,11 @@ def run(which: str, ranges, odom, params=None, laser=None, use_solver=True, tmpd
     np.savez(fin, ranges=ranges, odom=odom, pkeys=np.array(list(params.keys())), pvals=np.array(list(params.values()), dtype=np.float64),
              lkeys=np.array(list(laser.keys())), lvals=np.array(list(laser.values()), dtype=np.float64), use_solver=int(use_solver),
              map_resolution=float(map_resolution), publish_every=int(publish_every),
-             events=np.array([[e[0], e[1] == "remove_node", e[2] if len(e) > 2 else -1] for e in events], dtype=np.int64).reshape(-1, 3))
+             events=np.array([[e[0], e[1] == "remove_node", e[2] if len(e) > 2 else -1] for e in events], dtype=np.int64).reshape(-1, 3),
+             sensors=np.zeros(0, dtype=np.int64) if sensors is None else np.asarray(sensors, dtype=np.int64),
+             l2keys=np.array(list((laser2 or {}).keys())), l2vals=np.array(list((laser2 or {}).values()), dtype=np.float64),
+             l2steps=np.array([c[0] for c in laser2_changes], dtype=np.int64),
+             l2changes=np.array([json.dumps(c[1]) for c in laser2_changes]))
     env = dict(os.environ)
     r = subprocess.run([sys.executable, os.path.abspath(__file__), which, fin, fout], capture_output=True, text=True, env=env)
     if r.returncode != 0:
@@ -268,6 +303,18 @@ def make_trajectory(seed: int, n_scans: int, step: float = 0.5):
     drift = np.cumsum(np.column_stack([rng.normal(0, 0.004, (len(traj), 2)), rng.normal(0, 0.0015, len(traj))]), axis=0)
     odom = traj + drift
     return ranges, odom, traj
+
+
+def make_two_laser_trajectory(seed: int, n_scans: int, block: int = 6, step: float = 0.5):
+    """make_trajectory with a second laser: scans alternate between the two lasers in blocks of `block` (A / B / A ...), so that
+    the mapper meets a new sensor's first scan, and the second laser (TWO_LASER) has a shorter threshold, a larger minimum
+    range and a shorter maximum range.  Returns ranges, odom, truth, sensors (0 / 1 per scan)."""
+    ranges, odom, traj = make_trajectory(seed, n_scans, step)
+    sensors = (np.arange(len(ranges)) // block) % 2
+    return ranges, odom, traj, sensors
+
+
+TWO_LASER = dict(DEFAULT_LASER, min_range=0.3, max_range=20.0, range_threshold=8.0)
 
 
 def localization_inprocess(which: str, map_ranges, map_odom, loc_ranges, loc_odom, params: dict, loc_params: dict, laser: dict,
@@ -472,8 +519,11 @@ if __name__ == "__main__":
                                          int(z["publish_every"]) if "publish_every" in z.files else 0)
         else:
             events = [(int(e[0]), "remove_node", int(e[2])) if e[1] else (int(e[0]), "publish") for e in z["events"]]
+            two = "sensors" in z.files and len(z["l2keys"]) > 0
             out = run_inprocess(which, z["ranges"], z["odom"], params, laser, bool(int(z["use_solver"])), float(z["map_resolution"]),
-                                int(z["publish_every"]), events)
+                                int(z["publish_every"]), events, sensors=z["sensors"] if two else None,
+                                laser2={str(k): float(v) for k, v in zip(z["l2keys"], z["l2vals"])} if two else None,
+                                laser2_changes=[(int(i), json.loads(str(c))) for i, c in zip(z["l2steps"], z["l2changes"])] if two else ())
     finally:
         os.dup2(saved, 1)
     np.savez(fout, **out)

@@ -9,6 +9,7 @@
 #include <csignal>
 #include <cstdlib>
 #include <execinfo.h>
+#include <map>
 #include <memory>
 #include <string>
 #include <unistd.h>
@@ -32,11 +33,11 @@ struct Replay {
 };
 const char * kLaser = "laser0";
 
-// a new scan at the odometric pose, corrected pose = odometric pose (SlamToolbox::getLocalizedRangeScan)
-LocalizedRangeScan * make_scan(const double * ranges, int n, const double odom[3], int id)
+// a new scan of laser `sensor` at the odometric pose, corrected pose = odometric pose (SlamToolbox::getLocalizedRangeScan)
+LocalizedRangeScan * make_scan(const double * ranges, int n, const double odom[3], int id, const char * sensor = kLaser)
 {
   RangeReadingsVector rr(ranges, ranges + n);
-  LocalizedRangeScan * s = new LocalizedRangeScan(Name(kLaser), rr);
+  LocalizedRangeScan * s = new LocalizedRangeScan(Name(sensor), rr);
   Pose2 p(odom[0], odom[1], odom[2]);
   s->SetOdometricPose(p);
   s->SetCorrectedPose(p);
@@ -96,6 +97,27 @@ int krep_init_laser(double min_angle, double max_angle, double ang_res, double m
   l->SetAngularResolution(ang_res); l->SetRangeThreshold(range_threshold);
   l->SetOffsetPose(Pose2(0.0, 0.0, 0.0));
   SensorManager::GetInstance()->RegisterSensor(l);
+  return static_cast<int>(l->GetNumberOfRangeReadings());
+}
+
+// A second (third, ...) laser, as slam_toolbox makes one per scan frame id: registers laser `name` with these limits, or sets
+// the limits of the laser already registered under it (every later CreateFromScans reads them).  Returns the number of range
+// readings, -1 for the first laser's name (krep_init_laser registers it).
+int krep_laser(const char * name, double min_angle, double max_angle, double ang_res, double min_range, double max_range,
+               double range_threshold)
+{
+  static std::map<std::string, LaserRangeFinder *> lasers;   // the ones registered here (GetSensorByName throws on others)
+  if (std::strcmp(name, kLaser) == 0) return -1;
+  LaserRangeFinder *& l = lasers[name];
+  const bool fresh = l == nullptr;
+  if (fresh) {
+    l = LaserRangeFinder::CreateLaserRangeFinder(LaserRangeFinder_Custom, Name(name));
+    l->SetMinimumAngle(min_angle); l->SetMaximumAngle(max_angle);
+    l->SetAngularResolution(ang_res);
+    l->SetOffsetPose(Pose2(0.0, 0.0, 0.0));
+  }
+  l->SetMinimumRange(min_range); l->SetMaximumRange(max_range); l->SetRangeThreshold(range_threshold);
+  if (fresh) SensorManager::GetInstance()->RegisterSensor(l);
   return static_cast<int>(l->GetNumberOfRangeReadings());
 }
 
@@ -185,6 +207,15 @@ int krep_process(void * rp, const double * ranges, int n, const double odom[3], 
 {
   Replay * r = static_cast<Replay *>(rp);
   return run_scan(r, make_scan(ranges, n, odom, id), "krep_process",
+                  [r](LocalizedRangeScan * s, Matrix3 *) { return r->mapper.Process(s); }, nullptr, nullptr);
+}
+
+// krep_process on laser `sensor` (krep_laser): the mapper's multi-sensor path, where AddEdges links the first scan of a new
+// sensor to the other sensors' scans
+int krep_process_on(void * rp, const char * sensor, const double * ranges, int n, const double odom[3], int id)
+{
+  Replay * r = static_cast<Replay *>(rp);
+  return run_scan(r, make_scan(ranges, n, odom, id, sensor), "krep_process_on",
                   [r](LocalizedRangeScan * s, Matrix3 *) { return r->mapper.Process(s); }, nullptr, nullptr);
 }
 

@@ -64,6 +64,10 @@ class OgParams(C.Structure):
                 ("maximum_range", C.c_double), ("min_pass_through", C.c_uint32), ("occupancy_threshold", C.c_double)]
 
 
+class OgLaser(C.Structure):
+    _fields_ = [("range_threshold", C.c_double), ("minimum_range", C.c_double), ("maximum_range", C.c_double)]
+
+
 class OgInfo(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("stride", C.c_int32), ("offset", C.c_double * 2)]
 
@@ -148,6 +152,7 @@ def lib():
     L.b200og_destroy.argtypes = [C.c_void_p]
     L.b200og_set_stream.argtypes = [C.c_void_p, C.c_void_p]
     L.b200og_add_scans.argtypes = [C.c_void_p, C.POINTER(CScan), C.c_int32]
+    L.b200og_add_scans_lasers.argtypes = [C.c_void_p, C.POINTER(CScan), C.c_int32, C.POINTER(OgLaser)]
     L.b200og_clear_scans.argtypes = [C.c_void_p]
     L.b200og_num_scans.argtypes = [C.c_void_p]
     L.b200og_build.argtypes = [C.c_void_p, C.POINTER(OgInfo)]
@@ -583,6 +588,10 @@ class OccupancyGrid:
     or, keeping the scans resident in HBM between map updates:
 
         grid = OccupancyGrid(resolution, laser); grid.AddScans(block); grid.Build(); grid.AddScans(more); grid.Build()
+
+    The laser given to the constructor sets the default limits.  Scans of other lasers keep their own limits, as the
+    reference reads each scan's own laser: grid.AddScans(block, laser=block.laser), or
+    OccupancyGrid.CreateFromScans([block_a, block_b], resolution) with each block built with its own laser.
     """
 
     def __init__(self, resolution: float, laser: LaserRangeFinder | None = None, min_pass_through: int = 2,
@@ -595,12 +604,25 @@ class OccupancyGrid:
         _check(lib().b200og_create(C.byref(self.params), C.byref(self._h)))
 
     @staticmethod
-    def CreateFromScans(rScans: ScanBlock | None, resolution: float, min_pass_through: int = 2,
+    def CreateFromScans(rScans, resolution: float, min_pass_through: int = 2,
                         occupancy_threshold: float = 0.1) -> "OccupancyGrid | None":
-        if rScans is None or len(rScans) == 0:
+        """rScans = one ScanBlock (its laser for every scan), or a sequence of ScanBlocks, each scan with its own block's
+        laser (a map of several lasers).  None when there are no scans, like the reference's NULL."""
+        if rScans is None:
             return None
-        g = OccupancyGrid(resolution, rScans.laser, min_pass_through, occupancy_threshold)
-        g.AddScans(rScans)
+        if isinstance(rScans, ScanBlock):
+            if len(rScans) == 0:
+                return None
+            g = OccupancyGrid(resolution, rScans.laser, min_pass_through, occupancy_threshold)
+            g.AddScans(rScans)
+            g.Build()
+            return g
+        blocks = [b for b in rScans if len(b)]
+        if not blocks:
+            return None
+        g = OccupancyGrid(resolution, blocks[0].laser, min_pass_through, occupancy_threshold)
+        for b in blocks:
+            g.AddScans(b, laser=b.laser)
         g.Build()
         return g
 
@@ -618,8 +640,21 @@ class OccupancyGrid:
     def set_stream(self, cuda_stream: int):
         _check(lib().b200og_set_stream(self._h, C.c_void_p(cuda_stream)))
 
-    def AddScans(self, scans: ScanBlock):
-        _check(lib().b200og_add_scans(self._h, scans.c, len(scans)))
+    def AddScans(self, scans: ScanBlock, laser=None):
+        """Appends the block's scans to the store.  laser=None: the scans take the handle's default limits (the
+        constructor's laser).  laser=LaserRangeFinder (for example scans.laser): that laser's limits for every scan.  A
+        sequence of len(scans) LaserRangeFinders: one per scan."""
+        if laser is None:
+            _check(lib().b200og_add_scans(self._h, scans.c, len(scans)))
+            return
+        n = len(scans)
+        per_scan = [laser] * n if isinstance(laser, LaserRangeFinder) else list(laser)
+        if len(per_scan) != n:
+            raise ValueError(f"AddScans: {len(per_scan)} lasers for {n} scans")
+        arr = (OgLaser * max(n, 1))()
+        for i, l in enumerate(per_scan):
+            arr[i] = OgLaser(l.range_threshold, l.minimum_range, l.maximum_range)
+        _check(lib().b200og_add_scans_lasers(self._h, scans.c, n, arr))
 
     def ClearScans(self):
         _check(lib().b200og_clear_scans(self._h))

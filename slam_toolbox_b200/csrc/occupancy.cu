@@ -6,10 +6,13 @@
 //   ranges [B]      raw range readings of all stored scans, scan after scan
 //   points [B][2]   their unfiltered world-frame point readings (LocalizedRangeScan::GetPointReadings(false))
 //   sensor [S][2]   sensor position of every scan; start [S+1] = first beam of every scan
+//   laser [S][3]    {range threshold, minimum range, maximum range} of every scan's own laser: AddScan and Update read
+//                   pScan->GetLaserRangeFinder() per scan (Karto.h:6146-6151, :5646-5698), so one map may mix lasers
 //   pass, hits [height][stride] uint32 counters; cells [height][stride] uint8 states
 //
 // Kernels of one build (b200og_build):
-//   k_og_bbox    min / max over the sensor positions and the in-range points   (ComputeDimensions)
+//   k_og_bbox    min / max over the sensor positions and the in-range points   (ComputeDimensions); one warp per scan,
+//                so that every beam is tested against its own scan's limits
 //   k_og_trace   a warp takes 32 adjacent beams of a scan, one per lane, and runs the reference's integer
 //                Bresenham loop on them in lock step; equal cell indices of neighbouring lanes are merged
 //                into one RED.ADD of the run length (no return value) -- integer sums commute, so the
@@ -54,9 +57,9 @@ struct OgDev {
   const double * points;
   const double * sensor;
   const int32_t * start;
+  const double * laser;    // [nscans][3] range threshold, minimum range, maximum range of every scan
   int32_t nscans, maxbeams;
   int64_t beam0, nbeams;   // beams [beam0, nbeams) of the built scan range (absolute store indices)
-  double rt, minr, maxr;
   double scale, offx, offy;
   int32_t width, height, stride;
   uint32_t * pass;
@@ -76,29 +79,35 @@ __device__ __forceinline__ double warp_max(double v)
   return v;
 }
 
-// partial[block][4] = {min x, min y, max x, max y}; BoundingBox2 starts at +-999999999999999999.99999 (Karto.h:2845-2849)
+// partial[block][4] = {min x, min y, max x, max y}; BoundingBox2 starts at +-999999999999999999.99999 (Karto.h:2845-2849).
+// One warp per scan (grid-stride over the scans): its lanes walk the scan's beams with the scan's own range limits.  The
+// result is a min / max, so it does not depend on which warp saw which scan.
 __global__ void __launch_bounds__(kOgThreads) k_og_bbox(OgDev d, double * partial)
 {
   __shared__ double sm[4][kOgThreads / 32];
   const double big = 999999999999999999.99999;
   double mnx = big, mny = big, mxx = -big, mxy = -big;
-  const int64_t step = (int64_t)gridDim.x * blockDim.x, t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  for (int64_t i = d.beam0 + t0; i < d.nbeams; i += step) {
-    const double r = d.ranges[i];
-    if (r >= d.minr && r <= d.rt) {   // math::InRange (Math.h:123), LocalizedRangeScan::Update Karto.h:5662
-      const double x = d.points[2 * i], y = d.points[2 * i + 1];
-      if (x < mnx) mnx = x;   // MakeFloor / MakeCeil: strict comparisons, NaN never wins
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = (int64_t)gridDim.x * (kOgThreads / 32);
+  for (int64_t s = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); s < d.nscans; s += nwarps) {
+    const double rt = d.laser[3 * s], minr = d.laser[3 * s + 1];
+    for (int64_t i = d.start[s] + lane; i < d.start[s + 1]; i += 32) {
+      const double r = d.ranges[i];
+      if (r >= minr && r <= rt) {   // math::InRange (Math.h:123), LocalizedRangeScan::Update Karto.h:5662
+        const double x = d.points[2 * i], y = d.points[2 * i + 1];
+        if (x < mnx) mnx = x;   // MakeFloor / MakeCeil: strict comparisons, NaN never wins
+        if (y < mny) mny = y;
+        if (x > mxx) mxx = x;
+        if (y > mxy) mxy = y;
+      }
+    }
+    if (lane == 0) {   // m_BoundingBox.Add(scanPose.GetPosition()) Karto.h:5694
+      const double x = d.sensor[2 * s], y = d.sensor[2 * s + 1];
+      if (x < mnx) mnx = x;
       if (y < mny) mny = y;
       if (x > mxx) mxx = x;
       if (y > mxy) mxy = y;
     }
-  }
-  for (int64_t s = t0; s < d.nscans; s += step) {   // m_BoundingBox.Add(scanPose.GetPosition()) Karto.h:5694
-    const double x = d.sensor[2 * s], y = d.sensor[2 * s + 1];
-    if (x < mnx) mnx = x;
-    if (y < mny) mny = y;
-    if (x > mxx) mxx = x;
-    if (y > mxy) mxy = y;
   }
   mnx = warp_min(mnx); mny = warp_min(mny); mxx = warp_max(mxx); mxy = warp_max(mxy);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
@@ -125,10 +134,11 @@ __global__ void __launch_bounds__(kOgThreads) k_og_scan_box(OgDev d, int32_t fir
   const int64_t nwarps = (int64_t)gridDim.x * (kOgThreads / 32);
   for (int64_t k = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); k < count; k += nwarps) {
     const int32_t s = first + (int32_t)k;
+    const double rt = d.laser[3 * (size_t)s], minr = d.laser[3 * (size_t)s + 1];
     double mnx = big, mny = big, mxx = -big, mxy = -big;
     for (int64_t i = d.start[s] + lane; i < d.start[s + 1]; i += 32) {
       const double r = d.ranges[i];
-      if (r >= d.minr && r <= d.rt) {
+      if (r >= minr && r <= rt) {
         const double x = d.points[2 * i], y = d.points[2 * i + 1];
         if (x < mnx) mnx = x;
         if (y < mny) mny = y;
@@ -231,8 +241,8 @@ __global__ void __launch_bounds__(kOgThreads) k_og_box_union(const double * box,
 }
 
 // Store compaction (b200og_remove_scans): scan k0 + k of the compacted store is old scan src[k].  One warp per surviving scan
-// copies its beams from the old offsets (old_start) to the new ones (new_start), its sensor position, and its box while the
-// old scan had one, into the second set of buffers.  Sources and destinations are different allocations, so no thread can
+// copies its beams from the old offsets (old_start) to the new ones (new_start), its sensor position, its laser limits,
+// and its box while the old scan had one, into the second set of buffers.  Sources and destinations are different allocations, so no thread can
 // overwrite a value another one has not read yet.
 struct OgCompact {
   const int32_t * src;
@@ -243,10 +253,12 @@ struct OgCompact {
   const double * points;
   const double * sensor;
   const double * box;
+  const double * laser;
   double * ranges2;
   double * points2;
   double * sensor2;
   double * box2;
+  double * laser2;
 };
 
 __global__ void __launch_bounds__(kOgThreads) k_og_compact(OgCompact c)
@@ -262,6 +274,7 @@ __global__ void __launch_bounds__(kOgThreads) k_og_compact(OgCompact c)
     }
     if (lane == 0) reinterpret_cast<double2 *>(c.sensor2)[t] = reinterpret_cast<const double2 *>(c.sensor)[s];
     if (lane < 4 && s < c.nboxed) c.box2[4 * (size_t)t + lane] = c.box[4 * (size_t)s + lane];
+    if (lane < 3) c.laser2[3 * (size_t)t + lane] = c.laser[3 * (size_t)s + lane];
   }
 }
 
@@ -297,18 +310,19 @@ __global__ void __launch_bounds__(kOgThreads) k_og_trace(OgDev d)
   for (int64_t g = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); g < total; g += nwarps) {
     const int32_t scan = (int32_t)(g % d.nscans), beam = (int32_t)(g / d.nscans) * 32 + lane;
     const int32_t b0 = d.start[scan];
+    const double rt = d.laser[3 * scan], minr = d.laser[3 * scan + 1], maxr = d.laser[3 * scan + 2];   // warp-uniform
     int32_t x = 0, y = 0, dX = 0, dY = 0, ystep = 1, len = 0;
     bool steep = false, end_hit = false;
     int32_t end_key = -1;
     if (beam < d.start[scan + 1] - b0) {
       const int64_t i = (int64_t)b0 + beam;
       const double r = d.ranges[i];
-      if (!(r <= d.minr || r >= d.maxr || r != r)) {                    // ignored readings, Karto.h:6160
-        const bool valid_end = r < (d.rt - kTolerance);                 // Karto.h:6158
+      if (!(r <= minr || r >= maxr || r != r)) {                        // ignored readings, Karto.h:6160
+        const bool valid_end = r < (rt - kTolerance);                   // Karto.h:6158
         const double sx = d.sensor[2 * scan], sy = d.sensor[2 * scan + 1];
         double px = d.points[2 * i], py = d.points[2 * i + 1];
-        if (r >= d.rt) {                                                // trace up to the range threshold, Karto.h:6164-6171
-          const double ratio = d.rt / r;
+        if (r >= rt) {                                                  // trace up to the range threshold, Karto.h:6164-6171
+          const double ratio = rt / r;
           const double dx = px - sx, dy = py - sy;
           px = sx + ratio * dx;
           py = sy + ratio * dy;
@@ -412,6 +426,7 @@ struct b200og {
   bool own_stream = false;
   // scan store
   GrowBuf<double> d_ranges, d_points, d_sensor;
+  GrowBuf<double> d_laser;   // [S][3] every scan's own limits (the handle's params for scans added without a laser)
   GrowBuf<int32_t> d_start;
   std::vector<int32_t> start{0};
   int32_t maxbeams = 0;
@@ -420,7 +435,7 @@ struct b200og {
   int32_t nboxed = 0;
   bool boxes_auth = false;
   // compaction targets (b200og_remove_scans), swapped with the store's buffers after each compaction
-  GrowBuf<double> d_ranges2, d_points2, d_sensor2, d_box2;
+  GrowBuf<double> d_ranges2, d_points2, d_sensor2, d_box2, d_laser2;
   GrowBuf<int32_t> d_start2, d_src;
   // staging (two pinned halves, filled while the other one is in flight)
   double * stage[2] = {nullptr, nullptr};
@@ -533,13 +548,19 @@ void upload_rows(b200og * h, const b200_scan * scans, int32_t n, double * dst, i
     if (pending[k]) B200_CUDA(cudaEventSynchronize(h->stage_done[k]));
 }
 
-int add_scans(b200og * h, const b200_scan * scans, int32_t n)
+// lasers == NULL: every scan takes the handle's params as its limits
+int add_scans(b200og * h, const b200_scan * scans, int32_t n, const b200og_laser * lasers)
 {
   if (n < 0 || (n > 0 && !scans)) { set_last_error("b200og_add_scans: bad argument"); return B200_ERR_INVALID_ARG; }
   size_t add = 0;
   for (int32_t s = 0; s < n; ++s) {
     if (scans[s].n < 0 || (scans[s].n > 0 && (!scans[s].ranges || !scans[s].points_xy))) {
       set_last_error("b200_scan: NULL pointer or negative size");
+      return B200_ERR_INVALID_ARG;
+    }
+    if (lasers && !(std::isfinite(lasers[s].range_threshold) && std::isfinite(lasers[s].minimum_range) &&
+                    std::isfinite(lasers[s].maximum_range))) {
+      set_last_error("b200og_add_scans_lasers: non-finite laser limit");
       return B200_ERR_INVALID_ARG;
     }
     add += (size_t)scans[s].n;
@@ -553,10 +574,11 @@ int add_scans(b200og * h, const b200_scan * scans, int32_t n)
   h->d_ranges.ensure(old_beams + add, old_beams, h->stream);
   h->d_points.ensure(2 * (old_beams + add), 2 * old_beams, h->stream);
   h->d_sensor.ensure(2 * (old_scans + n), 2 * old_scans, h->stream);
+  h->d_laser.ensure(3 * (old_scans + n), 3 * old_scans, h->stream);
   h->d_start.ensure(old_scans + n + 1, old_scans, h->stream);   // entry old_scans is rewritten below
   upload_rows(h, scans, n, h->d_ranges.p + old_beams, 1, [](const b200_scan & s) { return s.ranges; });
   upload_rows(h, scans, n, h->d_points.p + 2 * old_beams, 2, [](const b200_scan & s) { return s.points_xy; });
-  // sensor positions + prefix of beam counts: small, staged in the first pinned half
+  // sensor positions, laser limits + prefix of beam counts: small, staged in the first pinned half
   double * sp = h->stage[0];
   std::vector<int32_t> st(n + 1);
   st[0] = (int32_t)old_beams;
@@ -564,11 +586,18 @@ int add_scans(b200og * h, const b200_scan * scans, int32_t n)
     st[s + 1] = st[s] + scans[s].n;
     h->maxbeams = std::max(h->maxbeams, scans[s].n);
   }
-  // (n sensor positions fit the 8 MB half up to 524,288 scans per call; larger calls go in slices)
-  for (int32_t s0 = 0; s0 < n; s0 += (int32_t)(kStageDoubles / 2)) {
-    const int32_t cnt = std::min<int32_t>(n - s0, (int32_t)(kStageDoubles / 2));
-    for (int32_t s = 0; s < cnt; ++s) { sp[2 * s] = scans[s0 + s].sensor_pose[0]; sp[2 * s + 1] = scans[s0 + s].sensor_pose[1]; }
+  // (n sensor positions and limits fit the 8 MB half up to 209,715 scans per call; larger calls go in slices)
+  constexpr int32_t kSlice = (int32_t)(kStageDoubles / 5);
+  for (int32_t s0 = 0; s0 < n; s0 += kSlice) {
+    const int32_t cnt = std::min<int32_t>(n - s0, kSlice);
+    double * lp = sp + 2 * (size_t)cnt;
+    for (int32_t s = 0; s < cnt; ++s) {
+      sp[2 * s] = scans[s0 + s].sensor_pose[0]; sp[2 * s + 1] = scans[s0 + s].sensor_pose[1];
+      const b200og_laser l = lasers ? lasers[s0 + s] : b200og_laser{h->p.range_threshold, h->p.minimum_range, h->p.maximum_range};
+      lp[3 * s] = l.range_threshold; lp[3 * s + 1] = l.minimum_range; lp[3 * s + 2] = l.maximum_range;
+    }
     B200_CUDA(cudaMemcpyAsync(h->d_sensor.p + 2 * (old_scans + s0), sp, 2 * (size_t)cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    B200_CUDA(cudaMemcpyAsync(h->d_laser.p + 3 * (old_scans + s0), lp, 3 * (size_t)cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     B200_CUDA(cudaStreamSynchronize(h->stream));
   }
   B200_CUDA(cudaMemcpyAsync(h->d_start.p + old_scans, st.data(), st.size() * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
@@ -583,6 +612,7 @@ OgDev range_view(const b200og * h, int32_t first, int32_t count)
 {
   OgDev d{};
   d.ranges = h->d_ranges.p; d.points = h->d_points.p; d.sensor = h->d_sensor.p + 2 * (size_t)first; d.start = h->d_start.p + first;
+  d.laser = h->d_laser.p + 3 * (size_t)first;
   d.nscans = count;
   d.beam0 = h->start[first]; d.nbeams = h->start[first + count];
   if (first == 0 && count == h->nscans()) {
@@ -590,7 +620,6 @@ OgDev range_view(const b200og * h, int32_t first, int32_t count)
   } else {
     for (int32_t s = first; s < first + count; ++s) d.maxbeams = std::max(d.maxbeams, h->start[s + 1] - h->start[s]);
   }
-  d.rt = h->p.range_threshold; d.minr = h->p.minimum_range; d.maxr = h->p.maximum_range;
   return d;
 }
 
@@ -703,6 +732,7 @@ int remove_scans(b200og * h, const int32_t * idx, int32_t n)
     h->d_ranges2.ensure(nbeams, 0, st);
     h->d_points2.ensure(2 * nbeams, 0, st);
     h->d_sensor2.ensure(2 * (size_t)S2, 0, st);
+    h->d_laser2.ensure(3 * (size_t)S2, 0, st);
     h->d_start2.ensure((size_t)S2 + 1, 0, st);
     h->d_src.ensure((size_t)count, 0, st);
     if (h->nboxed) h->d_box2.ensure(4 * (size_t)nboxed, 0, st);
@@ -711,12 +741,15 @@ int remove_scans(b200og * h, const int32_t * idx, int32_t n)
       B200_CUDA(cudaMemcpyAsync(h->d_ranges2.p, h->d_ranges.p, keep * sizeof(double), cudaMemcpyDeviceToDevice, st));
       B200_CUDA(cudaMemcpyAsync(h->d_points2.p, h->d_points.p, 2 * keep * sizeof(double), cudaMemcpyDeviceToDevice, st));
     }
-    if (k0) B200_CUDA(cudaMemcpyAsync(h->d_sensor2.p, h->d_sensor.p, 2 * (size_t)k0 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (k0) {
+      B200_CUDA(cudaMemcpyAsync(h->d_sensor2.p, h->d_sensor.p, 2 * (size_t)k0 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      B200_CUDA(cudaMemcpyAsync(h->d_laser2.p, h->d_laser.p, 3 * (size_t)k0 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    }
     if (kbox) B200_CUDA(cudaMemcpyAsync(h->d_box2.p, h->d_box.p, 4 * kbox * sizeof(double), cudaMemcpyDeviceToDevice, st));
     B200_CUDA(cudaMemcpyAsync(h->d_start2.p, start.data(), start.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaMemcpyAsync(h->d_src.p, src.data(), src.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     OgCompact c{h->d_src.p, h->d_start.p, h->d_start2.p, k0, count, h->nboxed, h->d_ranges.p, h->d_points.p, h->d_sensor.p,
-                h->d_box.p, h->d_ranges2.p, h->d_points2.p, h->d_sensor2.p, h->d_box2.p};
+                h->d_box.p, h->d_laser.p, h->d_ranges2.p, h->d_points2.p, h->d_sensor2.p, h->d_box2.p, h->d_laser2.p};
     const int nb = (int)std::min<int64_t>(((int64_t)count + kOgThreads / 32 - 1) / (kOgThreads / 32), (int64_t)h->sms * 8);
     B200_CUDA(cudaEventRecord(h->ev0, st));
     k_og_compact<<<nb, kOgThreads, 0, st>>>(c);
@@ -728,6 +761,7 @@ int remove_scans(b200og * h, const int32_t * idx, int32_t n)
     h->d_ranges.swap(h->d_ranges2);
     h->d_points.swap(h->d_points2);
     h->d_sensor.swap(h->d_sensor2);
+    h->d_laser.swap(h->d_laser2);
     h->d_start.swap(h->d_start2);
     if (h->nboxed) h->d_box.swap(h->d_box2);
   }
@@ -878,7 +912,15 @@ int b200og_add_scans(b200og * h, const b200_scan * scans, int32_t n)
 {
   B200_GUARD_BEGIN
   if (!h) return B200_ERR_INVALID_ARG;
-  return add_scans(h, scans, n);
+  return add_scans(h, scans, n, nullptr);
+  B200_GUARD_END
+}
+
+int b200og_add_scans_lasers(b200og * h, const b200_scan * scans, int32_t n, const b200og_laser * lasers)
+{
+  B200_GUARD_BEGIN
+  if (!h) return B200_ERR_INVALID_ARG;
+  return add_scans(h, scans, n, lasers);
   B200_GUARD_END
 }
 
@@ -992,7 +1034,7 @@ int b200og_create_from_scans(const b200og_params * params, const b200_scan * sca
   int rc = b200og_create(params, &raw);
   if (rc != B200_OK) return rc;
   std::unique_ptr<b200og, void (*)(b200og *)> h(raw, b200og_destroy);
-  rc = add_scans(h.get(), scans, n);
+  rc = add_scans(h.get(), scans, n, nullptr);
   if (rc == B200_OK) rc = build(h.get(), 0, h->nscans(), info);
   if (rc != B200_OK) return rc;
   *out = h.release();

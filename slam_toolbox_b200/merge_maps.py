@@ -80,11 +80,13 @@ class MergeMapsKinematic:
         self.locations: dict[int, np.ndarray] = {}         # submap_locations_: x, y, accumulated yaw
         self.corrections: dict[int, Transform] = {}        # submap_marker_transform_
 
-    def AddSubmap(self, block: api.ScanBlock):
+    def AddSubmap(self, block: api.ScanBlock, laser=None):
         """addSubmapCallback (:105-140): stores the scans, builds the submap's own grid from the shared store.  Returns
-        (id, nav map [height, width] int8, (x, y) of the submap frame) with the frame at the grid's centre (:115-122)."""
+        (id, nav map [height, width] int8, (x, y) of the submap frame) with the frame at the grid's centre (:115-122).
+        laser = the submap's own laser (each pose-graph file brings its own; a per-scan sequence is accepted too), None =
+        the tool's default laser given to the constructor."""
         first = self.grid.NumScans()
-        self.grid.AddScans(block)
+        self.grid.AddScans(block, laser)
         sid = len(self.ranges) + 1
         self.ranges[sid] = (first, len(block))
         self.grid.Build(first, len(block))
