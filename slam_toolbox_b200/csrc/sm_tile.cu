@@ -177,6 +177,9 @@ struct TileShared {
   double acc[4];
   int ok;
 };
+// The planner's shared-memory budget subtracts this size, and tests/tile_plan_rule.py restates the planner with it: a change here
+// changes plans, so it has to be made in both places.
+static_assert(sizeof(TileShared) == 1936, "TileShared changed size: update the planner restatement in tests/tile_plan_rule.py");
 
 // ------------------------------------------------------------------------------------------
 // section timers (build with -DB200_TILE_TIMERS, tools/tile_timers.py): lane 0 of every warp accumulates clock64() deltas
@@ -218,8 +221,10 @@ __device__ unsigned long long g_tile_timers[kTmCount];
 // the last y-tile the sixth register pair holds the tail row nY - 1, read lane-parallel over the entries (lane-row y_l takes every
 // 8th entry from the y_l-th on) and summed over the lane-rows at the flush.  A 2k + 1-row window (41, 81) then loads 40 k rows + an
 // eighth of a row per entry instead of 48 * ceil((2k + 1) / 48) rows.
+// f is __grid_constant__: the raster indexes its tap masks by the level at run time, which then reads the parameter bank instead
+// of a per-thread copy of TileDev.
 template <int kPitchW, bool kTail>
-__global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, TileDev f)
+__global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, const __grid_constant__ TileDev f)
 {
   constexpr int kMain = kTail ? kRowTiles - 1 : kRowTiles;   // row tiles of 8 rows per y-tile
   constexpr int kYTile = 8 * kMain;
@@ -303,43 +308,77 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, Tile
       const int ph = e.stage / nb, band = e.stage - ph * nb;
       const int pp = ph & 1, pq = ph >> 1;
       const int band_r0 = band * f.band_rows;
-      if (e.flags & kSeqNewChunk)
-        for (int i = tid; i < chunk_na * P; i += kTileThreads) A[i] = 0;
-      if (e.flags & kSeqNewStage) {
+      const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
+      if (e.flags & kSeqNewChunk) {
+        // A is 16-byte aligned (16 bytes behind the 16-byte aligned sub-grid); chunk_na * P need not be a multiple of 4
+        const int na = chunk_na * P, na4 = na >> 2;
+        uint4 * A4 = reinterpret_cast<uint4 *>(A);
+        for (int i = tid; i < na4; i += kTileThreads) A4[i] = zero4;
+        if (tid < (na & 3)) A[4 * na4 + tid] = 0;
+      }
+      if ((e.flags & (kSeqNewStage | kSeqKeepGrid)) == kSeqNewStage) {
         {
           uint4 * S4 = reinterpret_cast<uint4 *>(s_raw);
-          const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-          for (int i = tid; i < (sub_words >> 2); i += kTileThreads) S4[i] = zero;   // pitch_w is a multiple of 4
+          for (int i = tid; i < (sub_words >> 2); i += kTileThreads) S4[i] = zero4;   // pitch_w is a multiple of 4
         }
         __syncthreads();
-        // ---- raster: taps landing on (pp, pq) cells of this band (AddScan / SmearPoint, M.cpp:1080-1104, M.h:1152-1183);
-        //      one thread per valid point, only the kernel rows / columns of this phase's parity ----
+        // ---- raster: taps landing on (pp, pq) cells of this band (AddScan / SmearPoint, M.cpp:1080-1104, M.h:1152-1183) ----
         // Max-stamp without atomics when the kernel has few distinct values (3 x 3: {6, 25, 100}): one pass per value in ascending
         // order, plain byte stores (all writers of a pass store the same value, a later pass overwrites with a larger one), a
         // barrier between passes.  Neighbouring beams end in neighbouring cells, so a CAS loop on the shared 32-bit words
         // serialises up to 8 lanes per word; kernels with more values keep it.
         const int nlev = f.nlevels;
-        for (int lv = 0; lv < (nlev > 0 ? nlev : 1); ++lv) {
-          const uint32_t want = nlev > 0 ? f.level[lv] : 0u;
-          for (int it = it0; it < it1; ++it) {
-            const int32_t * cl = it == it0 ? cells0 : d.cells + (size_t)it * d.max_n;
-            const int ncell = it == it0 ? ncell0 : d.cell_count[it];
-            for (int t = tid; t < ncell; t += kTileThreads) {
-              const int32_t cell = cl[t];
-              if (cell < 0) continue;
-              const int cx = (cell & 0xFFFF) + d.roi_x - half, cy = (cell >> 16) + d.roi_y - half;
-              for (int ky = (cy ^ pq) & 1; ky < d.ksize; ky += 2) {
-                const int rel = ((cy + ky) >> 1) - band_r0;
-                if ((unsigned)rel >= (unsigned)f.alloc_rows) continue;
-                for (int kx = (cx ^ pp) & 1; kx < d.ksize; kx += 2) {
-                  const uint32_t kv = kern[ky * d.ksize + kx];
-                  if (nlev > 0) { if (kv == want) S8[rel * pitchB + ((cx + kx) >> 1)] = (uint8_t)kv; }
-                  else if (kv) atomic_max_u8(S8 + rel * pitchB + ((cx + kx) >> 1), kv);
+        if (f.tap_masks) {
+          // one thread per valid point: the pass's four class masks are warp-uniform parameter loads, a point selects its class's
+          // mask and stores one byte per set bit.  No table load and no compare per tap, and no tap is visited in a pass that
+          // does not store it.  (On H100 a raster still takes about as long as with the per-tap loop below: DESIGN.md §3.3)
+          for (int lv = 0; lv < nlev; ++lv) {
+            const uint8_t want = (uint8_t)f.level[lv];
+            const unsigned long long m0 = f.tap_mask[lv][0], m1 = f.tap_mask[lv][1], m2 = f.tap_mask[lv][2], m3 = f.tap_mask[lv][3];
+            for (int it = it0; it < it1; ++it) {
+              const int32_t * cl = it == it0 ? cells0 : d.cells + (size_t)it * d.max_n;
+              const int ncell = it == it0 ? ncell0 : d.cell_count[it];
+              for (int t = tid; t < ncell; t += kTileThreads) {
+                const int32_t cell = cl[t];
+                if (cell < 0) continue;
+                const int cx = (cell & 0xFFFF) + d.roi_x - half, cy = (cell >> 16) + d.roi_y - half;
+                const int ky0 = (cy ^ pq) & 1, kx0 = (cx ^ pp) & 1;
+                unsigned long long m = ky0 ? (kx0 ? m3 : m2) : (kx0 ? m1 : m0);
+                const int rel0 = ((cy + ky0) >> 1) - band_r0, col0 = (cx + kx0) >> 1;
+                while (m) {
+                  const int b = __ffsll((long long)m) - 1;
+                  m &= m - 1;
+                  const int rel = rel0 + (b >> 3);
+                  if ((unsigned)rel < (unsigned)f.alloc_rows) S8[rel * pitchB + col0 + (b & 7)] = want;
                 }
               }
             }
+            if (lv + 1 < nlev) __syncthreads();
           }
-          if (lv + 1 < nlev) __syncthreads();
+        } else {
+          // one thread per valid point, every kernel row / column of this phase's parity
+          for (int lv = 0; lv < (nlev > 0 ? nlev : 1); ++lv) {
+            const uint32_t want = nlev > 0 ? f.level[lv] : 0u;
+            for (int it = it0; it < it1; ++it) {
+              const int32_t * cl = it == it0 ? cells0 : d.cells + (size_t)it * d.max_n;
+              const int ncell = it == it0 ? ncell0 : d.cell_count[it];
+              for (int t = tid; t < ncell; t += kTileThreads) {
+                const int32_t cell = cl[t];
+                if (cell < 0) continue;
+                const int cx = (cell & 0xFFFF) + d.roi_x - half, cy = (cell >> 16) + d.roi_y - half;
+                for (int ky = (cy ^ pq) & 1; ky < d.ksize; ky += 2) {
+                  const int rel = ((cy + ky) >> 1) - band_r0;
+                  if ((unsigned)rel >= (unsigned)f.alloc_rows) continue;
+                  for (int kx = (cx ^ pp) & 1; kx < d.ksize; kx += 2) {
+                    const uint32_t kv = kern[ky * d.ksize + kx];
+                    if (nlev > 0) { if (kv == want) S8[rel * pitchB + ((cx + kx) >> 1)] = (uint8_t)kv; }
+                    else if (kv) atomic_max_u8(S8 + rel * pitchB + ((cx + kx) >> 1), kv);
+                  }
+                }
+              }
+            }
+            if (lv + 1 < nlev) __syncthreads();
+          }
         }
       }
       if (e.flags & (kSeqNewChunk | kSeqNewStage)) __syncthreads();
@@ -1129,6 +1168,16 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     if (!lv.empty() && lv[0] == 0) lv.erase(lv.begin());
     T.nlevels = (!lv.empty() && lv.size() <= 4) ? (int)lv.size() : 0;
     for (int i = 0; i < 4; ++i) T.level[i] = i < T.nlevels ? lv[i] : 0;
+    // the levelled raster's tap masks: for level l and class c = 2 ky0 + kx0 (the first kernel row / column of a point's phase
+    // parity), bit 8 dy + dx for the tap ky = ky0 + 2 dy, kx = kx0 + 2 dx of that value
+    const int ks = g.ksize;
+    T.tap_masks = (T.nlevels > 0 && ks <= kTileMaxMaskKsize) ? 1 : 0;
+    if (T.tap_masks)
+      for (int l = 0; l < T.nlevels; ++l)
+        for (int c = 0; c < 4; ++c)
+          for (int ky = c >> 1; ky < ks; ky += 2)
+            for (int kx = c & 1; kx < ks; kx += 2)
+              if (g.kernel[(size_t)ky * ks + kx] == T.level[l]) T.tap_mask[l][c] |= 1ull << (8 * (ky >> 1) + (kx >> 1));
   }
   T.off_A = s_bytes + 4 * kAGuardLo; T.off_probs = s_bytes + a_bytes; T.off_stage = (T.off_probs + probs_bytes + 127) & ~(size_t)127;
   T.off_cells = T.off_stage + 2 * (size_t)stage_bytes;
@@ -1224,7 +1273,11 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
       seq_start[(size_t)q * C + r] = (int32_t)seq.size();
       for (int v = r; v < V; v += C) {
         const int ca0 = v * nAc, cna = std::min(nAc, nA - ca0);
-        for (int sg = 0; sg < nstage; ++sg) {
+        // the CTA's chunks alternate the stage order (phase 0 -> 3, then 3 -> 0, ...): each chunk starts on the (phase, band) the
+        // one before it ended on, whose sub-grid is still resident
+        const bool backward = ((v - r) / C) & 1, keep = v != r;
+        for (int si = 0; si < nstage; ++si) {
+          const int sg = backward ? nstage - 1 - si : si;
           // sub-blocks: as many angles as fit one staging buffer
           int a = ca0;
           bool first_sub = true;
@@ -1272,7 +1325,8 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
             e.off = (int32_t)blob.size();
             e.bytes = (int32_t)bytes;
             e.chunk = (int16_t)v; e.stage = (int16_t)sg; e.a0 = (int16_t)a; e.nitems = (int16_t)items.size();
-            e.flags = (first_sub ? kSeqNewStage : 0u) | ((first_sub && sg == 0) ? kSeqNewChunk : 0u);
+            e.flags = (first_sub ? kSeqNewStage : 0u) | ((first_sub && si == 0) ? kSeqNewChunk : 0u) |
+                      ((first_sub && si == 0 && keep) ? kSeqKeepGrid : 0u);
             if (first_sub)
               for (int aa = ca0; aa < ca0 + cna; ++aa)
                 if (!cls[aa].wrap2[sg].empty()) e.flags |= kSeqHasWrap;

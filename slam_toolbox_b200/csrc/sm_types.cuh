@@ -167,7 +167,15 @@ struct TileSeq {                 // one descriptor block of a query's schedule (
 // (al < 64: the planner's nAc <= 63; np <= 640, ns <= 63, npairs <= 160: derived with the planner's refusal codes in sm_tile.cu,
 // and every record is checked against its field widths)
 constexpr int kItemMaxXTiles = 64, kItemMaxYTiles = 256;
-constexpr uint32_t kSeqNewChunk = 1, kSeqNewStage = 2, kSeqEndChunk = 4, kSeqHasWrap = 16;
+// kSeqNewStage marks the first block of every (chunk, stage): the stage's wrapped-EDGE and FAR passes run after it.  kSeqKeepGrid
+// on such a block says that the sub-grid of the block before it (the previous chunk's last stage) is the same (phase, band), so the
+// clear and the raster are skipped: the schedule runs a CTA's chunks in alternating stage order to make every chunk boundary so.
+constexpr uint32_t kSeqNewChunk = 1, kSeqNewStage = 2, kSeqEndChunk = 4, kSeqKeepGrid = 8, kSeqHasWrap = 16;
+// Levelled raster from tap masks: the taps of the smear kernel by (level, class), where a point's class in phase (pp, pq) is
+// c = 2 * ((cell row ^ pq) & 1) + ((cell column ^ pp) & 1) and picks the kernel rows / columns of that phase's parity.  Bit
+// 8 * dy + dx of a mask is the tap dy sub-grid rows / dx columns from the point's first cell of the phase, so a class holds at
+// most 8 x 8 taps: kernels up to kTileMaxMaskKsize wide.  Wider kernels keep the per-tap loop.
+constexpr int kTileMaxMaskKsize = 15;
 struct TileDev {
   int enabled;
   int C, V, nAc;                 // cluster size, angle chunks, angles per chunk
@@ -177,6 +185,8 @@ struct TileDev {
   int stage_bytes;               // size of one descriptor staging buffer
   int nlevels;                   // distinct non-zero smear-kernel values if <= 4 (levelled raster without atomics), else 0
   uint32_t level[4];             // ... ascending
+  int tap_masks;                 // the levelled raster stamps from tap_mask (nlevels > 0 and ksize <= kTileMaxMaskKsize)
+  unsigned long long tap_mask[4][4];   // [level][class]: the taps of that class with that value
   int int_ties;                  // responses are monotone in the integer sum with spacing > tolerance: integer arg-max / ties
   size_t off_A, off_probs, off_stage, off_cells;   // byte offsets into dynamic shared memory (S at 0)
   int cell_cap;                  // entries of one cell-list staging buffer (= max_n), 0 = cells are read from global memory
