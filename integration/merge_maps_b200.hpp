@@ -22,6 +22,7 @@
 
 #include "karto_sdk/Karto.h"
 #include "b200slam.h"
+#include "occupancy_b200.hpp"
 
 namespace karto {
 namespace b200 {
@@ -39,23 +40,12 @@ public:
   int AddSubmap(const LocalizedRangeScanVector & rScans, OccupancyGrid ** grid = nullptr)
   {
     if (grid) *grid = NULL;
-    std::vector<b200_scan> scans;
     std::vector<b200og_laser> lasers;
-    for (LocalizedRangeScan * s : rScans) {
-      if (s == nullptr) continue;                                   // Karto.h:6094, :6123
-      LaserRangeFinder * l = s->GetLaserRangeFinder();
-      if (!laser_) laser_ = l;
-      lasers.push_back(b200og_laser{l->GetRangeThreshold(), l->GetMinimumRange(), l->GetMaximumRange()});
-      b200_scan o;
-      const PointVectorDouble & pts = s->GetPointReadings(false);
-      o.n = static_cast<int32_t>(pts.size());
-      o.ranges = s->GetRangeReadings();
-      o.points_xy = reinterpret_cast<const double *>(pts.data());
-      const Pose2 p = s->GetSensorPose();
-      o.sensor_pose[0] = p.GetX(); o.sensor_pose[1] = p.GetY(); o.sensor_pose[2] = p.GetHeading();
-      scans.push_back(o);
+    const std::vector<b200_scan> scans = detail::CollectScans(rScans, &lasers, &laser_);
+    if (!h_) {
+      const b200og_params p = detail::GridParams(resolution_, laser_);
+      if (b200og_create(&p, &h_) != B200_OK) return Fail();
     }
-    if (!Ensure()) return -1;
     const int32_t first = b200og_num_scans(h_);
     if (b200og_add_scans_lasers(h_, scans.data(), static_cast<int32_t>(scans.size()), lasers.data()) != B200_OK) return Fail();
     submaps_.push_back({first, static_cast<int32_t>(scans.size())});
@@ -98,33 +88,12 @@ public:
 private:
   struct Range { int32_t first, count; };
 
-  bool Ensure()
-  {
-    if (h_) return true;
-    b200og_params p;
-    b200og_default_params(&p);                                      // MinPassThrough 2, OccupancyThreshold 0.1
-    p.resolution = resolution_;
-    if (laser_) {
-      p.range_threshold = laser_->GetRangeThreshold();
-      p.minimum_range = laser_->GetMinimumRange();
-      p.maximum_range = laser_->GetMaximumRange();
-    }
-    if (b200og_create(&p, &h_) != B200_OK) { Fail(); return false; }
-    return true;
-  }
-
   // the grid of scans [first, first + count)
   OccupancyGrid * Build(int32_t first, int32_t count)
   {
     b200og_info info;
     if (b200og_build_range(h_, first, count, &info) != B200_OK) { Fail(); return NULL; }
-    OccupancyGrid * g = new OccupancyGrid(info.width, info.height, Vector2<kt_double>(info.offset[0], info.offset[1]), resolution_);
-    if (g->GetWidthStep() != info.stride || b200og_fetch(h_, g->GetDataPointer(), nullptr, nullptr) != B200_OK) {
-      Fail();
-      delete g;
-      return NULL;
-    }
-    return g;
+    return detail::FetchGrid(h_, info, resolution_, "SubmapStore");
   }
 
   int Fail() const

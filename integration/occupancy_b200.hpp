@@ -81,12 +81,13 @@ inline b200og_params GridParams(kt_double resolution, LaserRangeFinder * laser)
   return p;
 }
 
-// the karto grid of a successful build of h
-inline OccupancyGrid * FetchGrid(b200og * h, const b200og_info & info, kt_double resolution)
+// the karto grid of a successful build of h; NULL, with the error printed under `who`, when it cannot be fetched
+inline OccupancyGrid * FetchGrid(b200og * h, const b200og_info & info, kt_double resolution,
+                                 const char * who = "OccupancyGrid::CreateFromScans")
 {
   OccupancyGrid * g = new OccupancyGrid(info.width, info.height, Vector2<kt_double>(info.offset[0], info.offset[1]), resolution);
   if (g->GetWidthStep() != info.stride || b200og_fetch(h, g->GetDataPointer(), nullptr, nullptr) != B200_OK) {
-    std::fprintf(stderr, "OccupancyGrid::CreateFromScans (b200): %s\n", b200_last_error());
+    std::fprintf(stderr, "%s (b200): %s\n", who, b200_last_error());
     delete g;
     g = NULL;
   }

@@ -167,11 +167,18 @@ def find_valid_points(scan, viewpoint):
 def occupancy(scans, resolution, range_threshold, minimum_range, maximum_range, min_pass_through=2,
               occupancy_threshold=0.1):
     """kp_occupancy_create on PortScan objects; same dict as oracle.karto_ref.occupancy (None when empty)."""
+    return occupancy_array(scan_array(scans), len(scans), resolution, range_threshold, minimum_range, maximum_range,
+                           min_pass_through, occupancy_threshold)
+
+
+def occupancy_array(arr, n, resolution, range_threshold, minimum_range, maximum_range, min_pass_through=2,
+                    occupancy_threshold=0.1):
+    """kp_occupancy_create on n KpScan records at arr (a KpScan array or pointer): dict(width, height, stride, offset,
+    cells, passes, hits, seconds), None when n is 0.  seconds is the host time of kp_occupancy_create."""
     import time
-    arr = scan_array(scans)
     t = time.perf_counter()
-    h = lib().kp_occupancy_create(arr, len(scans), resolution, range_threshold, minimum_range, maximum_range,
-                                  min_pass_through, occupancy_threshold)
+    h = lib().kp_occupancy_create(arr, n, resolution, range_threshold, minimum_range, maximum_range, min_pass_through,
+                                  occupancy_threshold)
     dt = time.perf_counter() - t
     if not h:
         return None

@@ -20,7 +20,8 @@ all: $(OUT)/libmerge_b200.so
 $(OUT)/merge_ref_driver.o: merge_ref_driver.cpp
 	@mkdir -p $(OUT)
 	$(CXX) $(CXXFLAGS) $(INC) -c $< -o $@
-$(OUT)/merge_maps_driver.o: $(INTEG)/merge_maps_driver.cpp $(INTEG)/merge_maps_b200.hpp ../include/b200slam.h
+$(OUT)/merge_maps_driver.o: $(INTEG)/merge_maps_driver.cpp $(INTEG)/merge_maps_b200.hpp $(INTEG)/occupancy_b200.hpp \
+                            ../include/b200slam.h
 	@mkdir -p $(OUT)
 	$(CXX) $(CXXFLAGS) $(INC) -c $< -o $@
 $(OUT)/libmerge_b200.so: $(OUT)/merge_maps_driver.o $(OUT)/merge_ref_driver.o $(OUT)/ref_driver.o $(OUT)/Karto.o $(OUT)/Mapper.o \

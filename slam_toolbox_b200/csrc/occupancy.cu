@@ -68,93 +68,84 @@ struct OgDev {
   int32_t * flag;          // set when a beam was refused (kOgMaxCells)
 };
 
-__device__ __forceinline__ double warp_min(double v)
+// BoundingBox2 (Karto.h:2845-2910), stored as {min x, min y, max x, max y}.  It starts at +-999999999999999999.99999, and
+// MakeFloor / MakeCeil compare strictly: NaN never wins, and of two equal values (-0.0 and +0.0) the first one added stays.
+// So every caller keeps the order of additions it has: the order decides which zero a box, and a grid offset, holds.
+struct OgBox {
+  static constexpr double kEmpty = 999999999999999999.99999;
+  double mnx = kEmpty, mny = kEmpty, mxx = -kEmpty, mxy = -kEmpty;
+
+  __host__ __device__ static OgBox load(const double * b) { return OgBox{b[0], b[1], b[2], b[3]}; }
+  __host__ __device__ void store(double * b) const { b[0] = mnx; b[1] = mny; b[2] = mxx; b[3] = mxy; }
+  __host__ __device__ void add(const OgBox & b)     // BoundingBox2::Add(BoundingBox2), Karto.h:2906-2910
+  {
+    if (b.mnx < mnx) mnx = b.mnx;
+    if (b.mny < mny) mny = b.mny;
+    if (b.mxx > mxx) mxx = b.mxx;
+    if (b.mxy > mxy) mxy = b.mxy;
+  }
+  __host__ __device__ void add(double x, double y) { add(OgBox{x, y, x, y}); }   // BoundingBox2::Add(Vector2), :2897-2901
+  // every lane of the warp ends with the union of the warp's boxes
+  __device__ void add_warp()
+  {
+    for (int o = 16; o; o >>= 1)
+      add(OgBox{__shfl_xor_sync(0xffffffffu, mnx, o), __shfl_xor_sync(0xffffffffu, mny, o), __shfl_xor_sync(0xffffffffu, mxx, o),
+                __shfl_xor_sync(0xffffffffu, mxy, o)});
+  }
+};
+
+// partial[block][4] = the union of every thread's box b: over each warp, then over the block's warps in order
+__device__ __forceinline__ void og_block_box(OgBox b, double * partial)
 {
-  for (int o = 16; o; o >>= 1) { double w = __shfl_xor_sync(0xffffffffu, v, o); v = w < v ? w : v; }
-  return v;
-}
-__device__ __forceinline__ double warp_max(double v)
-{
-  for (int o = 16; o; o >>= 1) { double w = __shfl_xor_sync(0xffffffffu, v, o); v = w > v ? w : v; }
-  return v;
+  __shared__ double sm[kOgThreads / 32][4];
+  b.add_warp();
+  if ((threadIdx.x & 31) == 0) b.store(sm[threadIdx.x >> 5]);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < kOgThreads / 32; ++k) b.add(OgBox::load(sm[k]));
+    b.store(partial + 4 * (size_t)blockIdx.x);
+  }
 }
 
-// partial[block][4] = {min x, min y, max x, max y}; BoundingBox2 starts at +-999999999999999999.99999 (Karto.h:2845-2849).
-// One warp per scan (grid-stride over the scans): its lanes walk the scan's beams with the scan's own range limits.  The
-// result is a min / max, so it does not depend on which warp saw which scan.
+// adds to b the points of scan s that this lane reads (beams lane, lane + 32, ...) and that are in the scan's own range
+// limits: math::InRange (Math.h:123) in LocalizedRangeScan::Update, Karto.h:5662
+__device__ __forceinline__ void og_add_scan_points(const OgDev & d, int64_t s, int lane, OgBox & b)
+{
+  const double rt = d.laser[3 * s], minr = d.laser[3 * s + 1];
+  for (int64_t i = d.start[s] + lane; i < d.start[s + 1]; i += 32) {
+    const double r = d.ranges[i];
+    if (r >= minr && r <= rt) b.add(d.points[2 * i], d.points[2 * i + 1]);
+  }
+}
+
+// partial[block][4] = the box of the block's scans.  One warp per scan (grid-stride over the scans): its lanes walk the scan's
+// beams with the scan's own range limits.  The result is a min / max, so it does not depend on which warp saw which scan.
 __global__ void __launch_bounds__(kOgThreads) k_og_bbox(OgDev d, double * partial)
 {
-  __shared__ double sm[4][kOgThreads / 32];
-  const double big = 999999999999999999.99999;
-  double mnx = big, mny = big, mxx = -big, mxy = -big;
+  OgBox b;
   const int lane = threadIdx.x & 31;
   const int64_t nwarps = (int64_t)gridDim.x * (kOgThreads / 32);
   for (int64_t s = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); s < d.nscans; s += nwarps) {
-    const double rt = d.laser[3 * s], minr = d.laser[3 * s + 1];
-    for (int64_t i = d.start[s] + lane; i < d.start[s + 1]; i += 32) {
-      const double r = d.ranges[i];
-      if (r >= minr && r <= rt) {   // math::InRange (Math.h:123), LocalizedRangeScan::Update Karto.h:5662
-        const double x = d.points[2 * i], y = d.points[2 * i + 1];
-        if (x < mnx) mnx = x;   // MakeFloor / MakeCeil: strict comparisons, NaN never wins
-        if (y < mny) mny = y;
-        if (x > mxx) mxx = x;
-        if (y > mxy) mxy = y;
-      }
-    }
-    if (lane == 0) {   // m_BoundingBox.Add(scanPose.GetPosition()) Karto.h:5694
-      const double x = d.sensor[2 * s], y = d.sensor[2 * s + 1];
-      if (x < mnx) mnx = x;
-      if (y < mny) mny = y;
-      if (x > mxx) mxx = x;
-      if (y > mxy) mxy = y;
-    }
+    og_add_scan_points(d, s, lane, b);
+    if (lane == 0) b.add(d.sensor[2 * s], d.sensor[2 * s + 1]);   // m_BoundingBox.Add(scanPose.GetPosition()) Karto.h:5694
   }
-  mnx = warp_min(mnx); mny = warp_min(mny); mxx = warp_max(mxx); mxy = warp_max(mxy);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { sm[0][w] = mnx; sm[1][w] = mny; sm[2][w] = mxx; sm[3][w] = mxy; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int k = 1; k < kOgThreads / 32; ++k) {
-      if (sm[0][k] < mnx) mnx = sm[0][k];
-      if (sm[1][k] < mny) mny = sm[1][k];
-      if (sm[2][k] > mxx) mxx = sm[2][k];
-      if (sm[3][k] > mxy) mxy = sm[3][k];
-    }
-    double * o = partial + 4 * (size_t)blockIdx.x;
-    o[0] = mnx; o[1] = mny; o[2] = mxx; o[3] = mxy;
-  }
+  og_block_box(b, partial);
 }
 
 // LocalizedRangeScan::Update's box of every scan in [first, first + count) (Karto.h:5662-5698): one warp per scan, the
-// in-range points and the sensor position, from BoundingBox2's +-999999999999999999.99999.  box[s] = {min x, min y, max x, max y}
+// in-range points and then the sensor position.  box[s] = {min x, min y, max x, max y}
 __global__ void __launch_bounds__(kOgThreads) k_og_scan_box(OgDev d, int32_t first, int32_t count, double * box)
 {
-  const double big = 999999999999999999.99999;
   const int lane = threadIdx.x & 31;
   const int64_t nwarps = (int64_t)gridDim.x * (kOgThreads / 32);
   for (int64_t k = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); k < count; k += nwarps) {
     const int32_t s = first + (int32_t)k;
-    const double rt = d.laser[3 * (size_t)s], minr = d.laser[3 * (size_t)s + 1];
-    double mnx = big, mny = big, mxx = -big, mxy = -big;
-    for (int64_t i = d.start[s] + lane; i < d.start[s + 1]; i += 32) {
-      const double r = d.ranges[i];
-      if (r >= minr && r <= rt) {
-        const double x = d.points[2 * i], y = d.points[2 * i + 1];
-        if (x < mnx) mnx = x;
-        if (y < mny) mny = y;
-        if (x > mxx) mxx = x;
-        if (y > mxy) mxy = y;
-      }
-    }
-    mnx = warp_min(mnx); mny = warp_min(mny); mxx = warp_max(mxx); mxy = warp_max(mxy);
+    OgBox b;
+    og_add_scan_points(d, s, lane, b);
+    b.add_warp();
     if (lane == 0) {
-      const double x = d.sensor[2 * s], y = d.sensor[2 * s + 1];
-      if (x < mnx) mnx = x;
-      if (y < mny) mny = y;
-      if (x > mxx) mxx = x;
-      if (y > mxy) mxy = y;
-      double * o = box + 4 * (size_t)s;
-      o[0] = mnx; o[1] = mny; o[2] = mxx; o[3] = mxy;
+      b.add(d.sensor[2 * s], d.sensor[2 * s + 1]);
+      b.store(box + 4 * (size_t)s);
     }
   }
 }
@@ -185,7 +176,6 @@ __global__ void __launch_bounds__(kOgThreads) k_og_transform(OgDev d, int32_t fi
     og_apply(t, points[2 * i], points[2 * i + 1], x, y);
     points[2 * i] = x; points[2 * i + 1] = y;
   }
-  const double big = 999999999999999999.99999;
   for (int64_t k = t0; k < count; k += step) {
     const int64_t s = first + k;
     if (do_sensor) {
@@ -195,70 +185,46 @@ __global__ void __launch_bounds__(kOgThreads) k_og_transform(OgDev d, int32_t fi
     }
     double * bx = box + 4 * s;
     const double cx[4] = {bx[0], bx[2], bx[2], bx[0]}, cy[4] = {bx[1], bx[3], bx[1], bx[3]};
-    double mnx = big, mny = big, mxx = -big, mxy = -big;
+    OgBox b;
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {   // BoundingBox2::Add, Karto.h:2897-2901
+    for (int c = 0; c < 4; ++c) {
       double x, y;
       og_apply(t, cx[c], cy[c], x, y);
-      if (x < mnx) mnx = x;
-      if (y < mny) mny = y;
-      if (x > mxx) mxx = x;
-      if (y > mxy) mxy = y;
+      b.add(x, y);
     }
-    bx[0] = mnx; bx[1] = mny; bx[2] = mxx; bx[3] = mxy;
+    b.store(bx);
   }
 }
 
-// ComputeDimensions over stored boxes (Karto.h:6097-6104, BoundingBox2::Add(BoundingBox2) :2906-2910): partial[block][4] like
-// k_og_bbox, the union of box[first .. first + count)
+// ComputeDimensions over stored boxes (Karto.h:6097-6104): partial[block][4] like k_og_bbox, the union of
+// box[first .. first + count)
 __global__ void __launch_bounds__(kOgThreads) k_og_box_union(const double * box, int32_t first, int32_t count, double * partial)
 {
-  __shared__ double sm[4][kOgThreads / 32];
-  const double big = 999999999999999999.99999;
-  double mnx = big, mny = big, mxx = -big, mxy = -big;
+  OgBox b;
   const int64_t step = (int64_t)gridDim.x * blockDim.x, t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  for (int64_t k = t0; k < count; k += step) {
-    const double * b = box + 4 * (first + k);
-    if (b[0] < mnx) mnx = b[0];
-    if (b[1] < mny) mny = b[1];
-    if (b[2] > mxx) mxx = b[2];
-    if (b[3] > mxy) mxy = b[3];
-  }
-  mnx = warp_min(mnx); mny = warp_min(mny); mxx = warp_max(mxx); mxy = warp_max(mxy);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { sm[0][w] = mnx; sm[1][w] = mny; sm[2][w] = mxx; sm[3][w] = mxy; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int k = 1; k < kOgThreads / 32; ++k) {
-      if (sm[0][k] < mnx) mnx = sm[0][k];
-      if (sm[1][k] < mny) mny = sm[1][k];
-      if (sm[2][k] > mxx) mxx = sm[2][k];
-      if (sm[3][k] > mxy) mxy = sm[3][k];
-    }
-    double * o = partial + 4 * (size_t)blockIdx.x;
-    o[0] = mnx; o[1] = mny; o[2] = mxx; o[3] = mxy;
-  }
+  for (int64_t k = t0; k < count; k += step) b.add(OgBox::load(box + 4 * (first + k)));
+  og_block_box(b, partial);
 }
 
-// Store compaction (b200og_remove_scans): scan k0 + k of the compacted store is old scan src[k].  One warp per surviving scan
-// copies its beams from the old offsets (old_start) to the new ones (new_start), its sensor position, its laser limits,
-// and its box while the old scan had one, into the second set of buffers.  Sources and destinations are different allocations, so no thread can
-// overwrite a value another one has not read yet.
+// The scan store's arrays on the device (OgStore::dev): ranges [B], points [B][2], sensor [S][2], laser [S][3], box [S][4]
+// (scans [0, nboxed) only), start [S + 1]
+struct OgStoreDev {
+  double * ranges;
+  double * points;
+  double * sensor;
+  double * laser;
+  double * box;
+  int32_t * start;
+};
+
+// Store compaction (b200og_remove_scans): scan k0 + k of the compacted store `to` is scan src[k] of `from`.  One warp per
+// surviving scan copies its beams from their offsets in `from` to their offsets in `to`, its sensor position, its laser
+// limits, and its box while the old scan had one.  `from` and `to` are different allocations, so no thread can overwrite a
+// value another one has not read yet.
 struct OgCompact {
   const int32_t * src;
-  const int32_t * old_start;
-  const int32_t * new_start;
   int32_t k0, count, nboxed;
-  const double * ranges;
-  const double * points;
-  const double * sensor;
-  const double * box;
-  const double * laser;
-  double * ranges2;
-  double * points2;
-  double * sensor2;
-  double * box2;
-  double * laser2;
+  OgStoreDev from, to;
 };
 
 __global__ void __launch_bounds__(kOgThreads) k_og_compact(OgCompact c)
@@ -267,14 +233,14 @@ __global__ void __launch_bounds__(kOgThreads) k_og_compact(OgCompact c)
   const int64_t nwarps = (int64_t)gridDim.x * (kOgThreads / 32);
   for (int64_t k = (int64_t)blockIdx.x * (kOgThreads / 32) + (threadIdx.x >> 5); k < c.count; k += nwarps) {
     const int32_t s = c.src[k], t = c.k0 + (int32_t)k;
-    const int32_t from = c.old_start[s], to = c.new_start[t], nb = c.old_start[s + 1] - from;
+    const int32_t from = c.from.start[s], to = c.to.start[t], nb = c.from.start[s + 1] - from;
     for (int32_t b = lane; b < nb; b += 32) {
-      c.ranges2[to + b] = c.ranges[from + b];
-      reinterpret_cast<double2 *>(c.points2)[to + b] = reinterpret_cast<const double2 *>(c.points)[from + b];
+      c.to.ranges[to + b] = c.from.ranges[from + b];
+      reinterpret_cast<double2 *>(c.to.points)[to + b] = reinterpret_cast<const double2 *>(c.from.points)[from + b];
     }
-    if (lane == 0) reinterpret_cast<double2 *>(c.sensor2)[t] = reinterpret_cast<const double2 *>(c.sensor)[s];
-    if (lane < 4 && s < c.nboxed) c.box2[4 * (size_t)t + lane] = c.box[4 * (size_t)s + lane];
-    if (lane < 3) c.laser2[3 * (size_t)t + lane] = c.laser[3 * (size_t)s + lane];
+    if (lane == 0) reinterpret_cast<double2 *>(c.to.sensor)[t] = reinterpret_cast<const double2 *>(c.from.sensor)[s];
+    if (lane < 4 && s < c.nboxed) c.to.box[4 * (size_t)t + lane] = c.from.box[4 * (size_t)s + lane];
+    if (lane < 3) c.to.laser[3 * (size_t)t + lane] = c.from.laser[3 * (size_t)s + lane];
   }
 }
 
@@ -413,7 +379,45 @@ struct GrowBuf {
     p = q;
     cap = want;
   }
+  void copy_from(const GrowBuf & o, size_t n, cudaStream_t st)   // the first n values of o
+  {
+    if (n) B200_CUDA(cudaMemcpyAsync(p, o.p, n * sizeof(T), cudaMemcpyDeviceToDevice, st));
+  }
   void swap(GrowBuf & o) { std::swap(p, o.p); std::swap(cap, o.cap); }
+};
+
+// The scan store's device arrays (layout at OgStoreDev).  The box array is sized apart from the others: boxes are made
+// lazily (ensure_boxes), and only scans [0, nboxed) have one.
+struct OgStore {
+  GrowBuf<double> ranges, points, sensor;
+  GrowBuf<double> laser;   // every scan's own limits (the handle's params for scans added without a laser)
+  GrowBuf<double> box;
+  GrowBuf<int32_t> start;
+
+  // room for `beams` beams and `scans` scans, keeping the first keep_beams beams and keep_scans scans (start: entries)
+  void ensure(size_t beams, size_t scans, size_t keep_beams, size_t keep_scans, cudaStream_t st)
+  {
+    ranges.ensure(beams, keep_beams, st);
+    points.ensure(2 * beams, 2 * keep_beams, st);
+    sensor.ensure(2 * scans, 2 * keep_scans, st);
+    laser.ensure(3 * scans, 3 * keep_scans, st);
+    start.ensure(scans + 1, keep_scans, st);
+  }
+  // the first `beams` beams, `scans` scans and `boxes` boxes of o; start is not copied
+  void copy_from(const OgStore & o, size_t beams, size_t scans, size_t boxes, cudaStream_t st)
+  {
+    ranges.copy_from(o.ranges, beams, st);
+    points.copy_from(o.points, 2 * beams, st);
+    sensor.copy_from(o.sensor, 2 * scans, st);
+    laser.copy_from(o.laser, 3 * scans, st);
+    box.copy_from(o.box, 4 * boxes, st);
+  }
+  void swap(OgStore & o, bool with_box)
+  {
+    ranges.swap(o.ranges); points.swap(o.points); sensor.swap(o.sensor); laser.swap(o.laser); start.swap(o.start);
+    if (with_box) box.swap(o.box);
+  }
+  OgStoreDev dev() const { return OgStoreDev{ranges.p, points.p, sensor.p, laser.p, box.p, start.p}; }
 };
 
 }  // namespace b200
@@ -424,19 +428,14 @@ struct b200og {
   b200og_params p{};
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  // scan store
-  GrowBuf<double> d_ranges, d_points, d_sensor;
-  GrowBuf<double> d_laser;   // [S][3] every scan's own limits (the handle's params for scans added without a laser)
-  GrowBuf<int32_t> d_start;
+  // scan store, and the compaction target (b200og_remove_scans) it is swapped with after each compaction
+  OgStore store, spare;
+  GrowBuf<int32_t> d_src;
   std::vector<int32_t> start{0};
   int32_t maxbeams = 0;
   // merge state: per-scan boxes of scans [0, nboxed), authoritative once a transform ran (boxes_auth)
-  GrowBuf<double> d_box;
   int32_t nboxed = 0;
   bool boxes_auth = false;
-  // compaction targets (b200og_remove_scans), swapped with the store's buffers after each compaction
-  GrowBuf<double> d_ranges2, d_points2, d_sensor2, d_box2, d_laser2;
-  GrowBuf<int32_t> d_start2, d_src;
   // staging (two pinned halves, filled while the other one is in flight)
   double * stage[2] = {nullptr, nullptr};
   cudaEvent_t stage_done[2] = {nullptr, nullptr};
@@ -467,6 +466,25 @@ struct b200og {
     }
   }
   int32_t nscans() const { return (int32_t)start.size() - 1; }
+  // blocks of a one-warp-per-scan kernel over `count` scans: at most 8 per SM, grid-stride beyond that
+  int scan_blocks(int64_t count) const
+  {
+    return (int)std::max<int64_t>(std::min<int64_t>((count + kOgThreads / 32 - 1) / (kOgThreads / 32), (int64_t)sms * 8), 1);
+  }
+  // after each launch: its error, and b200og_launch_count
+  void launched()
+  {
+    B200_CUDA(cudaGetLastError());
+    ++launches;
+  }
+  // b200og_kernel_ms = the device time between timer_start and timer_stop; timer_stop waits for the stream
+  void timer_start() { B200_CUDA(cudaEventRecord(ev0, stream)); }
+  void timer_stop()
+  {
+    B200_CUDA(cudaEventRecord(ev1, stream));
+    B200_CUDA(cudaStreamSynchronize(stream));
+    B200_CUDA(cudaEventElapsedTime(&last_ms, ev0, ev1));
+  }
 };
 
 namespace {
@@ -571,13 +589,10 @@ int add_scans(b200og * h, const b200_scan * scans, int32_t n, const b200og_laser
   h->ensure_stream();
   for (auto & sp : h->stage)
     if (!sp) sp = stage_pool().take();
-  h->d_ranges.ensure(old_beams + add, old_beams, h->stream);
-  h->d_points.ensure(2 * (old_beams + add), 2 * old_beams, h->stream);
-  h->d_sensor.ensure(2 * (old_scans + n), 2 * old_scans, h->stream);
-  h->d_laser.ensure(3 * (old_scans + n), 3 * old_scans, h->stream);
-  h->d_start.ensure(old_scans + n + 1, old_scans, h->stream);   // entry old_scans is rewritten below
-  upload_rows(h, scans, n, h->d_ranges.p + old_beams, 1, [](const b200_scan & s) { return s.ranges; });
-  upload_rows(h, scans, n, h->d_points.p + 2 * old_beams, 2, [](const b200_scan & s) { return s.points_xy; });
+  OgStore & d = h->store;
+  d.ensure(old_beams + add, old_scans + n, old_beams, old_scans, h->stream);   // start entry old_scans is rewritten below
+  upload_rows(h, scans, n, d.ranges.p + old_beams, 1, [](const b200_scan & s) { return s.ranges; });
+  upload_rows(h, scans, n, d.points.p + 2 * old_beams, 2, [](const b200_scan & s) { return s.points_xy; });
   // sensor positions, laser limits + prefix of beam counts: small, staged in the first pinned half
   double * sp = h->stage[0];
   std::vector<int32_t> st(n + 1);
@@ -596,11 +611,11 @@ int add_scans(b200og * h, const b200_scan * scans, int32_t n, const b200og_laser
       const b200og_laser l = lasers ? lasers[s0 + s] : b200og_laser{h->p.range_threshold, h->p.minimum_range, h->p.maximum_range};
       lp[3 * s] = l.range_threshold; lp[3 * s + 1] = l.minimum_range; lp[3 * s + 2] = l.maximum_range;
     }
-    B200_CUDA(cudaMemcpyAsync(h->d_sensor.p + 2 * (old_scans + s0), sp, 2 * (size_t)cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    B200_CUDA(cudaMemcpyAsync(h->d_laser.p + 3 * (old_scans + s0), lp, 3 * (size_t)cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    B200_CUDA(cudaMemcpyAsync(d.sensor.p + 2 * (old_scans + s0), sp, 2 * (size_t)cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    B200_CUDA(cudaMemcpyAsync(d.laser.p + 3 * (old_scans + s0), lp, 3 * (size_t)cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     B200_CUDA(cudaStreamSynchronize(h->stream));
   }
-  B200_CUDA(cudaMemcpyAsync(h->d_start.p + old_scans, st.data(), st.size() * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(d.start.p + old_scans, st.data(), st.size() * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   h->start.insert(h->start.end(), st.begin() + 1, st.end());
   h->built = false;
@@ -611,8 +626,9 @@ int add_scans(b200og * h, const b200_scan * scans, int32_t n, const b200og_laser
 OgDev range_view(const b200og * h, int32_t first, int32_t count)
 {
   OgDev d{};
-  d.ranges = h->d_ranges.p; d.points = h->d_points.p; d.sensor = h->d_sensor.p + 2 * (size_t)first; d.start = h->d_start.p + first;
-  d.laser = h->d_laser.p + 3 * (size_t)first;
+  const OgStore & s = h->store;
+  d.ranges = s.ranges.p; d.points = s.points.p; d.sensor = s.sensor.p + 2 * (size_t)first; d.start = s.start.p + first;
+  d.laser = s.laser.p + 3 * (size_t)first;
   d.nscans = count;
   d.beam0 = h->start[first]; d.nbeams = h->start[first + count];
   if (first == 0 && count == h->nscans()) {
@@ -638,13 +654,11 @@ void ensure_boxes(b200og * h)
   const int32_t n = h->nscans();
   if (h->nboxed == n) return;
   h->ensure_stream();
-  h->d_box.ensure(4 * (size_t)n, 4 * (size_t)h->nboxed, h->stream);
+  h->store.box.ensure(4 * (size_t)n, 4 * (size_t)h->nboxed, h->stream);
   const OgDev d = range_view(h, 0, n);
   const int32_t count = n - h->nboxed;
-  const int nb = (int)std::min<int64_t>(((int64_t)count + kOgThreads / 32 - 1) / (kOgThreads / 32), (int64_t)h->sms * 8);
-  k_og_scan_box<<<std::max(nb, 1), kOgThreads, 0, h->stream>>>(d, h->nboxed, count, h->d_box.p);
-  B200_CUDA(cudaGetLastError());
-  ++h->launches;
+  k_og_scan_box<<<h->scan_blocks(count), kOgThreads, 0, h->stream>>>(d, h->nboxed, count, h->store.box.p);
+  h->launched();
   h->nboxed = n;
 }
 
@@ -662,7 +676,7 @@ int transform_scans(b200og * h, int32_t first, int32_t count, const double * bas
   if (sensor_poses) {   // host-computed sensor poses (lasers with a mounting offset): positions only
     std::vector<double> xy(2 * (size_t)count);
     for (int32_t s = 0; s < count; ++s) { xy[2 * s] = sensor_poses[3 * s]; xy[2 * s + 1] = sensor_poses[3 * s + 1]; }
-    B200_CUDA(cudaMemcpyAsync(h->d_sensor.p + 2 * (size_t)first, xy.data(), xy.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(h->store.sensor.p + 2 * (size_t)first, xy.data(), xy.size() * sizeof(double), cudaMemcpyHostToDevice, st));
   }
   OgTf t;
   for (int r = 0; r < 2; ++r) {
@@ -672,14 +686,11 @@ int transform_scans(b200og * h, int32_t first, int32_t count, const double * bas
   const OgDev d = range_view(h, first, count);
   const int64_t work = std::max<int64_t>(d.nbeams - d.beam0, count);
   const int nb = (int)std::min<int64_t>((work + kOgThreads - 1) / kOgThreads, (int64_t)h->sms * 8);
-  B200_CUDA(cudaEventRecord(h->ev0, st));
-  k_og_transform<<<std::max(nb, 1), kOgThreads, 0, st>>>(d, first, count, t, sensor_poses ? 0 : 1, h->d_points.p, h->d_sensor.p,
-                                                         h->d_box.p);
-  B200_CUDA(cudaGetLastError());
-  ++h->launches;
-  B200_CUDA(cudaEventRecord(h->ev1, st));
-  B200_CUDA(cudaStreamSynchronize(st));   // the host staging of sensor_poses is released on return
-  B200_CUDA(cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+  h->timer_start();
+  k_og_transform<<<std::max(nb, 1), kOgThreads, 0, st>>>(d, first, count, t, sensor_poses ? 0 : 1, h->store.points.p,
+                                                         h->store.sensor.p, h->store.box.p);
+  h->launched();
+  h->timer_stop();   // the host staging of sensor_poses is released on return
   h->boxes_auth = true;
   h->built = false;
   return B200_OK;
@@ -693,7 +704,7 @@ int scan_boxes(b200og * h, int32_t first, int32_t count, double * boxes)
   }
   if (count == 0) return B200_OK;
   ensure_boxes(h);
-  B200_CUDA(cudaMemcpyAsync(boxes, h->d_box.p + 4 * (size_t)first, 4 * (size_t)count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpyAsync(boxes, h->store.box.p + 4 * (size_t)first, 4 * (size_t)count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200_OK;
 }
@@ -729,41 +740,19 @@ int remove_scans(b200og * h, const int32_t * idx, int32_t n)
     cudaStream_t st = h->stream;
     const size_t keep = (size_t)start[k0], nbeams = (size_t)start[S2], kbox = (size_t)std::min(k0, h->nboxed);
     const int32_t count = (int32_t)src.size();
-    h->d_ranges2.ensure(nbeams, 0, st);
-    h->d_points2.ensure(2 * nbeams, 0, st);
-    h->d_sensor2.ensure(2 * (size_t)S2, 0, st);
-    h->d_laser2.ensure(3 * (size_t)S2, 0, st);
-    h->d_start2.ensure((size_t)S2 + 1, 0, st);
+    h->spare.ensure(nbeams, (size_t)S2, 0, 0, st);
     h->d_src.ensure((size_t)count, 0, st);
-    if (h->nboxed) h->d_box2.ensure(4 * (size_t)nboxed, 0, st);
-    // the scans before the first removed one keep their offsets: plain copies into the second buffers
-    if (keep) {
-      B200_CUDA(cudaMemcpyAsync(h->d_ranges2.p, h->d_ranges.p, keep * sizeof(double), cudaMemcpyDeviceToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->d_points2.p, h->d_points.p, 2 * keep * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    }
-    if (k0) {
-      B200_CUDA(cudaMemcpyAsync(h->d_sensor2.p, h->d_sensor.p, 2 * (size_t)k0 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-      B200_CUDA(cudaMemcpyAsync(h->d_laser2.p, h->d_laser.p, 3 * (size_t)k0 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    }
-    if (kbox) B200_CUDA(cudaMemcpyAsync(h->d_box2.p, h->d_box.p, 4 * kbox * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(h->d_start2.p, start.data(), start.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (h->nboxed) h->spare.box.ensure(4 * (size_t)nboxed, 0, st);
+    // the scans before the first removed one keep their offsets: plain copies into the spare store
+    h->spare.copy_from(h->store, keep, (size_t)k0, kbox, st);
+    B200_CUDA(cudaMemcpyAsync(h->spare.start.p, start.data(), start.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaMemcpyAsync(h->d_src.p, src.data(), src.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    OgCompact c{h->d_src.p, h->d_start.p, h->d_start2.p, k0, count, h->nboxed, h->d_ranges.p, h->d_points.p, h->d_sensor.p,
-                h->d_box.p, h->d_laser.p, h->d_ranges2.p, h->d_points2.p, h->d_sensor2.p, h->d_box2.p, h->d_laser2.p};
-    const int nb = (int)std::min<int64_t>(((int64_t)count + kOgThreads / 32 - 1) / (kOgThreads / 32), (int64_t)h->sms * 8);
-    B200_CUDA(cudaEventRecord(h->ev0, st));
-    k_og_compact<<<nb, kOgThreads, 0, st>>>(c);
-    B200_CUDA(cudaGetLastError());
-    ++h->launches;
-    B200_CUDA(cudaEventRecord(h->ev1, st));
-    B200_CUDA(cudaStreamSynchronize(st));   // start and src are released on return
-    B200_CUDA(cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
-    h->d_ranges.swap(h->d_ranges2);
-    h->d_points.swap(h->d_points2);
-    h->d_sensor.swap(h->d_sensor2);
-    h->d_laser.swap(h->d_laser2);
-    h->d_start.swap(h->d_start2);
-    if (h->nboxed) h->d_box.swap(h->d_box2);
+    const OgCompact c{h->d_src.p, k0, count, h->nboxed, h->store.dev(), h->spare.dev()};
+    h->timer_start();
+    k_og_compact<<<h->scan_blocks(count), kOgThreads, 0, st>>>(c);
+    h->launched();
+    h->timer_stop();   // start and src are released on return
+    h->store.swap(h->spare, h->nboxed > 0);
   }
   // removing only trailing scans moves nothing: the device prefix up to the new end is unchanged
   h->start.swap(start);
@@ -789,30 +778,22 @@ int build(b200og * h, int32_t first, int32_t count, b200og_info * info)
   h->h_partial.reserve(4 * (size_t)blocks);
   h->d_flag.reserve(1);
   h->h_flag.reserve(1);
-  B200_CUDA(cudaEventRecord(h->ev0, st));
+  h->timer_start();
   if (h->boxes_auth) {   // transformed store: the union of the stored boxes (ComputeDimensions reads them, IsDirty is clear)
     ensure_boxes(h);
-    k_og_box_union<<<blocks, kOgThreads, 0, st>>>(h->d_box.p, first, count, h->d_partial.p);
+    k_og_box_union<<<blocks, kOgThreads, 0, st>>>(h->store.box.p, first, count, h->d_partial.p);
   } else {
     k_og_bbox<<<blocks, kOgThreads, 0, st>>>(d, h->d_partial.p);
   }
-  B200_CUDA(cudaGetLastError());
-  ++h->launches;
+  h->launched();
   B200_CUDA(cudaMemcpyAsync(h->h_partial.p, h->d_partial.p, 4 * (size_t)blocks * sizeof(double), cudaMemcpyDeviceToHost, st));
   B200_CUDA(cudaStreamSynchronize(st));
-  const double big = 999999999999999999.99999;
-  double mnx = big, mny = big, mxx = -big, mxy = -big;
-  for (int b = 0; b < blocks; ++b) {
-    const double * o = h->h_partial.p + 4 * (size_t)b;
-    if (o[0] < mnx) mnx = o[0];
-    if (o[1] < mny) mny = o[1];
-    if (o[2] > mxx) mxx = o[2];
-    if (o[3] > mxy) mxy = o[3];
-  }
+  OgBox box;
+  for (int b = 0; b < blocks; ++b) box.add(OgBox::load(h->h_partial.p + 4 * (size_t)b));
   // ComputeDimensions, Karto.h:6100-6106
   const double scale = 1.0 / h->p.resolution;
-  const int32_t width = to_int32(round_half_away((mxx - mnx) * scale));
-  const int32_t height = to_int32(round_half_away((mxy - mny) * scale));
+  const int32_t width = to_int32(round_half_away((box.mxx - box.mnx) * scale));
+  const int32_t height = to_int32(round_half_away((box.mxy - box.mny) * scale));
   if (width < 0 || height < 0) { set_last_error("OccupancyGrid: bounding box of the scans is not finite"); return B200_ERR_UNSUPPORTED; }
   const int64_t stride = ((int64_t)width + 7) & ~(int64_t)7;   // Karto.h:4640
   const int64_t ncells = stride * height;
@@ -821,12 +802,12 @@ int build(b200og * h, int32_t first, int32_t count, b200og_info * info)
     return B200_ERR_UNSUPPORTED;
   }
   h->info.width = width; h->info.height = height; h->info.stride = (int32_t)stride;
-  h->info.offset[0] = mnx; h->info.offset[1] = mny;
+  h->info.offset[0] = box.mnx; h->info.offset[1] = box.mny;
   const size_t cells = (size_t)ncells;
   h->d_pass.reserve(cells + 4);
   h->d_hits.reserve(cells + 4);
   h->d_cells.reserve(cells + 4);
-  d.scale = scale; d.offx = mnx; d.offy = mny;
+  d.scale = scale; d.offx = box.mnx; d.offy = box.mny;
   d.width = width; d.height = height; d.stride = (int32_t)stride;
   d.pass = h->d_pass.p; d.hits = h->d_hits.p; d.cells = h->d_cells.p; d.flag = h->d_flag.p;
   B200_CUDA(cudaMemsetAsync(h->d_flag.p, 0, sizeof(int32_t), st));
@@ -834,17 +815,14 @@ int build(b200og * h, int32_t first, int32_t count, b200og_info * info)
     B200_CUDA(cudaMemsetAsync(h->d_pass.p, 0, cells * sizeof(uint32_t), st));
     B200_CUDA(cudaMemsetAsync(h->d_hits.p, 0, cells * sizeof(uint32_t), st));
     k_og_trace<<<blocks, kOgThreads, 0, st>>>(d);
-    B200_CUDA(cudaGetLastError());
+    h->launched();
     const size_t quads = cells / 4;   // stride is a multiple of 8
     const int ub = (int)std::min<size_t>((quads + kOgThreads - 1) / kOgThreads, (size_t)h->sms * 16);
     k_og_update<<<std::max(ub, 1), kOgThreads, 0, st>>>(d, h->p.min_pass_through, h->p.occupancy_threshold, quads);
-    B200_CUDA(cudaGetLastError());
-    h->launches += 2;
+    h->launched();
   }
   B200_CUDA(cudaMemcpyAsync(h->h_flag.p, h->d_flag.p, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  B200_CUDA(cudaEventRecord(h->ev1, st));
-  B200_CUDA(cudaStreamSynchronize(st));
-  B200_CUDA(cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+  h->timer_stop();
   if (h->h_flag.p[0]) {
     set_last_error("OccupancyGrid: a beam spans more than 2^24 cells (corrupt pose or resolution)");
     return B200_ERR_UNSUPPORTED;
@@ -1006,8 +984,7 @@ int b200og_fetch_nav(b200og * h, int8_t * data)
     h->d_nav.reserve(n);
     const int nb = (int)std::min<size_t>((n + kOgThreads - 1) / kOgThreads, (size_t)h->sms * 16);
     k_og_nav<<<nb, kOgThreads, 0, h->stream>>>(h->d_cells.p, h->info.width, h->info.height, h->info.stride, h->d_nav.p);
-    B200_CUDA(cudaGetLastError());
-    ++h->launches;
+    h->launched();
     B200_CUDA(cudaMemcpyAsync(data, h->d_nav.p, n, cudaMemcpyDeviceToHost, h->stream));
     B200_CUDA(cudaStreamSynchronize(h->stream));
   }

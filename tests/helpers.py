@@ -131,18 +131,8 @@ def port_occupancy(rec, res, rt, mp=2, th=0.1):
     import ctypes as C
     from oracle import karto_port as P
     assert C.sizeof(P.KpScan) == SCAN_DTYPE.itemsize
-    h = P.lib().kp_occupancy_create(rec.ctypes.data_as(C.POINTER(P.KpScan)), len(rec), res, rt, LASER["min_range"],
-                                    LASER["max_range"], int(mp), th)
-    info = (C.c_int32 * 3)()
-    off = np.zeros(2)
-    P.lib().kp_occupancy_info(h, info, off.ctypes.data_as(C.POINTER(C.c_double)))
-    w, hh, st = info[0], info[1], info[2]
-    n = hh * st
-    grab = lambda f, t: np.ctypeslib.as_array(f(h), shape=(max(n, 1),))[:n].reshape(hh, st).astype(t, copy=True)   # noqa: E731
-    out = dict(width=w, height=hh, stride=st, offset=off, cells=grab(P.lib().kp_occupancy_cells, np.uint8),
-               passes=grab(P.lib().kp_occupancy_pass, np.uint32), hits=grab(P.lib().kp_occupancy_hits, np.uint32))
-    P.lib().kp_occupancy_destroy(h)
-    return out
+    return P.occupancy_array(rec.ctypes.data_as(C.POINTER(P.KpScan)), len(rec), res, rt, LASER["min_range"], LASER["max_range"],
+                             int(mp), th)
 
 
 def occupancy_params(params):

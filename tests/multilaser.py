@@ -179,17 +179,7 @@ def host_occupancy(ranges, points, poses, lasers, res, min_pass_through=2, occup
         for i, s in enumerate(members):
             arr[i] = P.KpScan(ranges.shape[1], ranges[s].ctypes.data_as(_DP), points[s].ctypes.data_as(_DP), (C.c_double * 3)(*poses[s]))
         arr[len(members)], arr[len(members) + 1] = anchors
-        h = P.lib().kp_occupancy_create(arr, len(members) + 2, res, lim[0], lim[1], lim[2], min_pass_through, occupancy_threshold)
-        info = (C.c_int32 * 3)()
-        off = np.zeros(2)
-        P.lib().kp_occupancy_info(h, info, off.ctypes.data_as(_DP))
-        w, hh, st = info[0], info[1], info[2]
-        n = hh * st
-
-        def grab(fn):
-            return np.ctypeslib.as_array(fn(h), shape=(max(n, 1),))[:n].reshape(hh, st).astype(np.uint32, copy=True)
-        g = dict(width=w, height=hh, stride=st, offset=off, passes=grab(P.lib().kp_occupancy_pass), hits=grab(P.lib().kp_occupancy_hits))
-        P.lib().kp_occupancy_destroy(h)
+        g = P.occupancy_array(arr, len(members) + 2, res, lim[0], lim[1], lim[2], min_pass_through, occupancy_threshold)
         if total is None:
             total = g
         else:

@@ -115,16 +115,11 @@ def test_ragged_scans_and_all_readings_ignored():
     for s in range(6):
         parr[s] = P.KpScan(len(rr[s]), keep[2 * s].ctypes.data_as(C.POINTER(C.c_double)), keep[2 * s + 1].ctypes.data_as(C.POINTER(C.c_double)),
                            (C.c_double * 3)(*run["poses"][s]))
-    hnd = P.lib().kp_occupancy_create(parr, 6, 0.05, 12.0, 0.1, 30.0, 2, 0.1)
-    info = (C.c_int32 * 3)(); off = np.zeros(2)
-    P.lib().kp_occupancy_info(hnd, info, off.ctypes.data_as(C.POINTER(C.c_double)))
-    n = info[1] * info[2]
-    exp_cells = np.ctypeslib.as_array(P.lib().kp_occupancy_cells(hnd), shape=(n,)).reshape(info[1], info[2]).copy()
-    exp_pass = np.ctypeslib.as_array(P.lib().kp_occupancy_pass(hnd), shape=(n,)).reshape(info[1], info[2]).copy()
-    P.lib().kp_occupancy_destroy(hnd)
+    exp = P.occupancy_array(parr, 6, 0.05, 12.0, 0.1, 30.0, 2, 0.1)
     got = as_dict(g)
-    assert (got["width"], got["height"], got["stride"]) == (info[0], info[1], info[2]) and np.array_equal(got["offset"], off)
-    assert np.array_equal(got["passes"], exp_pass) and np.array_equal(got["cells"], exp_cells)
+    assert (got["width"], got["height"], got["stride"]) == (exp["width"], exp["height"], exp["stride"])
+    assert np.array_equal(got["offset"], exp["offset"])
+    assert np.array_equal(got["passes"], exp["passes"]) and np.array_equal(got["cells"], exp["cells"])
 
 
 def test_full_size_map_properties():

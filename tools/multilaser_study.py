@@ -5,8 +5,11 @@ occupancy_grid workload: make_mapping_run(3, 5000) in a 60 m world).
              upload's host wall time.  A third store holds every scan through b200og_add_scans_lasers with the first laser's
              limits, so that the cost of per-scan limits is told apart from the cost of the other laser's different work.
   parent   : the existing workload (one laser, b200og_add_scans + b200og_build) on the parent commit's library and on this
-             tree's, alternated round by round in one process; both libraries are driven through the same C calls
-Medians of `--builds` builds per round, over `--rounds` rounds; the spread is (max - min) / median of the round medians.
+             tree's, alternated round by round in one process; both libraries are driven through the same C calls.  The same
+             store then takes `--builds` compactions (b200og_remove_scans of its first scan, so every other scan moves) and
+             `--builds` transforms of every scan (b200og_transform_scans), each timed by b200og_kernel_ms, and a last build
+             of the compacted, transformed store whose output must be identical too.
+Medians of `--builds` calls per round, over `--rounds` rounds; the spread is (max - min) / median of the round medians.
 Writes the JSON to the path given (default profiles/h100_multilaser.json).  Card name and power limit are read in the run.
     python tools/multilaser_study.py [out.json] [--parent-lib build/parent/libb200slam.so] [--rounds 7] [--builds 20]"""
 import argparse
@@ -47,6 +50,10 @@ def bind(L):
     L.b200og_build.argtypes = [C.c_void_p, C.POINTER(api.OgInfo)]
     L.b200og_kernel_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
     L.b200og_fetch.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+    L.b200og_remove_scans.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]
+    L.b200og_num_scans.argtypes = [C.c_void_p]
+    L.b200og_transform_scans.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                         C.POINTER(C.c_double)]
     return L
 
 
@@ -58,6 +65,28 @@ def builds(L, h, n):
         L.b200og_kernel_ms(h, C.byref(ms))
         out.append(ms.value)
     return out, info
+
+
+def timed(L, h, n, call):
+    """b200og_kernel_ms of n calls of call()"""
+    ms, out = C.c_float(), []
+    for _ in range(n):
+        assert call() == 0
+        L.b200og_kernel_ms(h, C.byref(ms))
+        out.append(ms.value)
+    return out
+
+
+def compactions(L, h, n):
+    first = (C.c_int32 * 1)(0)
+    return timed(L, h, n, lambda: L.b200og_remove_scans(h, first, 1))
+
+
+def transforms(L, h, n):
+    t = 0.001   # a small rotation and shift per call, so that the grid keeps its size
+    basis = (C.c_double * 9)(np.cos(t), -np.sin(t), 0.0, np.sin(t), np.cos(t), 0.0, 0.0, 0.0, 1.0)
+    origin = (C.c_double * 3)(0.01, -0.005, 0.0)
+    return timed(L, h, n, lambda: L.b200og_transform_scans(h, 0, L.b200og_num_scans(h), basis, origin, None))
 
 
 def one_laser_store(L, block):
@@ -125,20 +154,30 @@ def main():
     # the existing workload: parent library against this tree's, alternated
     if os.path.exists(a.parent_lib):
         libs = {"parent": bind(C.CDLL(a.parent_lib)), "change": bind(C.CDLL(api.library_path()))}
-        rounds = {k: [] for k in libs}
-        digests = {}
+        rounds = {op: {k: [] for k in libs} for op in ("occupancy_grid", "compaction", "transform")}
+        digests = {op: {} for op in ("occupancy_grid", "after_compaction_and_transform")}
         for r in range(a.rounds):
             for k in (("parent", "change") if r % 2 == 0 else ("change", "parent")):
                 L = libs[k]
                 h = one_laser_store(L, block)
                 ms, info = builds(L, h, a.builds)
-                rounds[k].append(ms)
+                rounds["occupancy_grid"][k].append(ms)
                 if r == 0:
-                    digests[k] = digest(L, h, info)
+                    digests["occupancy_grid"][k] = digest(L, h, info)
+                rounds["compaction"][k].append(compactions(L, h, a.builds))
+                rounds["transform"][k].append(transforms(L, h, a.builds))
+                if r == 0:
+                    info = api.OgInfo()
+                    assert L.b200og_build(h, C.byref(info)) == 0
+                    digests["after_compaction_and_transform"][k] = digest(L, h, info)
                 L.b200og_destroy(h)
-        res["occupancy_grid"] = {k: summary(v) for k, v in rounds.items()}
-        res["occupancy_grid"]["identical_output"] = digests["parent"] == digests["change"]
-        res["occupancy_grid"]["change_over_parent"] = res["occupancy_grid"]["change"]["median_ms"] / res["occupancy_grid"]["parent"]["median_ms"]
+        for op, v in rounds.items():
+            res[op] = {k: summary(x) for k, x in v.items()}
+            res[op]["change_over_parent"] = res[op]["change"]["median_ms"] / res[op]["parent"]["median_ms"]
+        res["occupancy_grid"]["identical_output"] = digests["occupancy_grid"]["parent"] == digests["occupancy_grid"]["change"]
+        res["compaction"]["identical_output"] = (digests["after_compaction_and_transform"]["parent"] ==
+                                                 digests["after_compaction_and_transform"]["change"])
+        res["transform"]["identical_output"] = res["compaction"]["identical_output"]
     else:
         res["occupancy_grid"] = dict(error=f"no parent library at {a.parent_lib}")
     os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
