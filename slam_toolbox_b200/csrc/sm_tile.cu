@@ -122,8 +122,13 @@ __device__ __forceinline__ void red_add(uint32_t a, uint32_t v)
   asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
 }
 
-__device__ __forceinline__ uint32_t even_bytes_t(uint32_t w) { return __byte_perm(w, 0, 0x4240); }   // [b0, 0, b2, 0]
+// Wrapped-word accumulation.  The item loops add every loaded word whole into Tw and only its odd bytes into To (uint32, mod
+// 2^32).  Every word is w = even(w) + (odd(w) << 8) with even(w) = [b0, 0, b2, 0], and k * w = k * even(w) + ((k * odd(w)) << 8)
+// mod 2^32, so Tw - (To << 8) is the sum of the even bytes mod 2^32 -- the even-field word E the loops would form by extracting
+// both halves -- for any words and weights.  One byte extract per loaded word instead of two.  (That E and To hold their 16-bit
+// fields without carries is the item's weight cap, kChunkBeams beams of cell values <= 100, as before.)
 __device__ __forceinline__ uint32_t odd_bytes_t(uint32_t w) { return __byte_perm(w, 0, 0x4341); }    // [b1, 0, b3, 0]
+__device__ __forceinline__ uint32_t even_fields(uint32_t tw, uint32_t to) { return tw - (to << 8); } // [sum b0 | sum b2]
 
 // best / tie summary of a set of poses (one chunk, one CTA, or the whole pair)
 struct TieRes {
@@ -210,6 +215,25 @@ __device__ unsigned long long g_tile_timers[kTmCount];
 #define TILE_TM(sec) do {} while (0)
 #define TILE_TM_END do {} while (0)
 #endif
+// loop-trip counters (build with -DB200_TILE_COUNTS, tools/tile_loop_account.py): lane 0 of every warp counts the items, the
+// flushes that reduce something and the trips of each correlation loop (lane 0 is lane-row 0, which runs the most tail-row trips,
+// so its count is the warp's).  Kept apart from the section timers: the counting itself costs correlation cycles.
+#ifdef B200_TILE_COUNTS
+enum { kCnItem, kCnFlush, kCnPlain4, kCnPlain2, kCnPlain1, kCnSingle, kCnPair, kCnTailPlain, kCnTailSingle, kCnTailPair, kCnEdge,
+       kCnCount };
+__device__ unsigned long long g_tile_counts[kCnCount];
+#define TILE_CN_DECL unsigned long long cn_acc[kCnCount] = {};
+#define TILE_CN(k) (++cn_acc[k])
+#define TILE_CN_END                                                                \
+  do {                                                                             \
+    if (lane == 0)                                                                 \
+      for (int s = 0; s < kCnCount; ++s) atomicAdd(&g_tile_counts[s], cn_acc[s]); \
+  } while (0)
+#else
+#define TILE_CN_DECL
+#define TILE_CN(k) do {} while (0)
+#define TILE_CN_END do {} while (0)
+#endif
 
 // ------------------------------------------------------------------------------------------
 // the kernel
@@ -248,6 +272,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
   const uint32_t bar0 = smem_u32(&sh.bar[0]);
   const uint32_t stg0 = smem_u32(s_raw + f.off_stage);
   TILE_TM_DECL
+  TILE_CN_DECL
 
   if (tid == 0) {
     mbar_init(bar0, 1);
@@ -401,6 +426,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
         if (lane == 0) item = atomicAdd(&sh.ctr[cnt & 1], 1);
         item = __shfl_sync(0xffffffffu, item, 0);
         if (item >= e.nitems) break;
+        TILE_CN(kCnItem);
         const uint2 rec = items[item];
         const int b0 = (int)(rec.x & 0xFFFFu);
         int b = b0;
@@ -428,32 +454,34 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
         // stay warp-uniform (LDS [R + UR]).
         const int x0 = 4 * (4 * xt + j_l) - m;
         // The flush is straight-line code: every lane reduces all of its fields, and a field that is not a pose of this item adds
-        // zero.  The lane's four x-range tests are fixed for the item and become masks of the two packed words (T0 holds the
-        // fields of x0 and x0 + 2, T1 those of x0 + 1 and x0 + 3); a row beyond the last pose row is masked to zero and its
+        // zero.  The lane's four x-range tests are fixed for the item and become masks of the two packed words (the even fields
+        // hold x0 and x0 + 2, the odd fields x0 + 1 and x0 + 3); a row beyond the last pose row is masked to zero and its
         // address clamped to the last one.  Columns -3 .. nX + 17 of a row stay inside the angle's volume or the guard words
         // around A (kAGuardLo / kAGuardHi), so every address is one the item may add zero to.
-        auto add4 = [&](uint32_t a, uint32_t t0, uint32_t t1) {
-          red_add(a + 0, t0 & 0xFFFFu);
-          red_add(a + 4, t1 & 0xFFFFu);
-          red_add(a + 8, t0 >> 16);
-          red_add(a + 12, t1 >> 16);
+        auto add4 = [&](uint32_t a, uint32_t te, uint32_t to) {
+          red_add(a + 0, te & 0xFFFFu);
+          red_add(a + 4, to & 0xFFFFu);
+          red_add(a + 8, te >> 16);
+          red_add(a + 12, to >> 16);
         };
-        auto flush = [&](const uint32_t (&T0)[kRowTiles], const uint32_t (&T1)[kRowTiles]) {
+        // Tw / To: wrapped whole-word and odd-byte sums of every row tile (even_fields above)
+        auto flush = [&](const uint32_t (&Tw)[kRowTiles], const uint32_t (&To)[kRowTiles]) {
           TILE_TM(kTmCorr);
-          uint32_t any = 0;
+          uint32_t any = 0;   // Tw = To = 0 exactly when E = To = 0 (E = Tw - (To << 8))
 #pragma unroll
-          for (int r = 0; r < kRowTiles; ++r) any |= T0[r] | T1[r];
+          for (int r = 0; r < kRowTiles; ++r) any |= Tw[r] | To[r];
           if (!__any_sync(0xffffffffu, any != 0)) { TILE_TM(kTmFlush); return; }
-          // the tail row's fields of the 8 lane-rows of a word column: three butterfly adds (the item's whole weight fits 16 bits)
-          // ahead of the first reduction, so that no convergence check splits the reductions.  Zero outside the last y-tile, so
-          // every item of the tail layout runs it unbranched.
-          uint32_t t0 = 0, t1 = 0;
+          TILE_CN(kCnFlush);
+          // the tail row's sums over the 8 lane-rows of a word column: three butterfly adds of Tw and To (E of a sum is the sum
+          // of the Es; the item's whole weight fits 16 bits) ahead of the first reduction, so that no convergence check
+          // splits the reductions.  Zero outside the last y-tile, so every item of the tail layout runs it unbranched.
+          uint32_t tw = 0, to = 0;
           if (kTail) {
-            t0 = T0[kRowTiles - 1]; t1 = T1[kRowTiles - 1];
+            tw = Tw[kRowTiles - 1]; to = To[kRowTiles - 1];
 #pragma unroll
             for (int o = 4; o < 32; o <<= 1) {
-              t0 += __shfl_xor_sync(0xffffffffu, t0, o);
-              t1 += __shfl_xor_sync(0xffffffffu, t1, o);
+              tw += __shfl_xor_sync(0xffffffffu, tw, o);
+              to += __shfl_xor_sync(0xffffffffu, to, o);
             }
           }
           const uint32_t xm0 = ((unsigned)x0 < (unsigned)nX ? 0x0000FFFFu : 0u) | ((unsigned)(x0 + 2) < (unsigned)nX ? 0xFFFF0000u : 0u);
@@ -464,23 +492,24 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
           for (int r = 0; r < kMain; ++r) {
             const int y = ybase + 8 * r;
             const uint32_t rm = y < y_end ? ~0u : 0u;
-            add4(ax + rowB * (uint32_t)min(y, ylast), T0[r] & xm0 & rm, T1[r] & xm1 & rm);
+            add4(ax + rowB * (uint32_t)min(y, ylast), even_fields(Tw[r], To[r]) & xm0 & rm, To[r] & xm1 & rm);
           }
           if (kTail) {
             // lane-row 0 (ybase == kYTile * yt) adds the tail row, the other lane-rows add zero to rows of their own (no
             // same-address atomics)
             const bool tv = tail && ybase == kYTile * yt;
             const uint32_t tm = tv ? ~0u : 0u;
-            add4(ax + rowB * (uint32_t)(tv ? nY - 1 : min(ybase, ylast)), t0 & xm0 & tm, t1 & xm1 & tm);
+            add4(ax + rowB * (uint32_t)(tv ? nY - 1 : min(ybase, ylast)), even_fields(tw, to) & xm0 & tm, to & xm1 & tm);
           }
           TILE_TM(kTmFlush);
         };
         // an item's plain and weighted beams weigh at most kChunkBeams (the host splits longer groups): one flush
         if (b < se || ps < pe2) {
-          uint32_t T0[kRowTiles], T1[kRowTiles];
+          uint32_t Tw[kRowTiles], To[kRowTiles];
 #pragma unroll
-          for (int r = 0; r < kRowTiles; ++r) { T0[r] = 0; T1[r] = 0; }
-          for (; b + 3 < pe; b += 4) {   // 4 beams: one broadcast LDS.64 of descriptors, two byte-wise pair sums, one 3-input add per field
+          for (int r = 0; r < kRowTiles; ++r) { Tw[r] = 0; To[r] = 0; }
+          for (; b + 3 < pe; b += 4) {   // 4 beams: one broadcast LDS.64 of descriptors, two byte-wise pair sums, one 3-input add per sum
+            TILE_CN(kCnPlain4);
             const uint2 dd = *reinterpret_cast<const uint2 *>(pay + b);
             // 16-bit word offsets -> byte addresses: one PRMT (half-word extract) + one shift-add each
             const uint32_t o0 = base + 4u * __byte_perm(dd.x, 0, 0x4410), o1 = base + 4u * __byte_perm(dd.x, 0, 0x4432);
@@ -491,46 +520,50 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
                                   lds_u32(o1 + r * 8 * pitchB);
               const uint32_t wb = lds_u32(o2 + r * 8 * pitchB) +
                                   lds_u32(o3 + r * 8 * pitchB);
-              T0[r] = T0[r] + even_bytes_t(wa) + even_bytes_t(wb);
-              T1[r] = T1[r] + odd_bytes_t(wa) + odd_bytes_t(wb);
+              Tw[r] = Tw[r] + wa + wb;
+              To[r] = To[r] + odd_bytes_t(wa) + odd_bytes_t(wb);
             }
           }
           for (; b + 1 < pe; b += 2) {
+            TILE_CN(kCnPlain2);
             const uint32_t dd = *reinterpret_cast<const uint32_t *>(pay + b);
             const uint32_t o0 = base + ((dd & 0xFFFFu) << 2), o1 = base + ((dd >> 16) << 2);
 #pragma unroll
             for (int r = 0; r < kMain; ++r) {
               const uint32_t w = lds_u32(o0 + r * 8 * pitchB) +
                                  lds_u32(o1 + r * 8 * pitchB);
-              T0[r] += even_bytes_t(w);
-              T1[r] += odd_bytes_t(w);
+              Tw[r] += w;
+              To[r] += odd_bytes_t(w);
             }
           }
           if (b < pe) {
+            TILE_CN(kCnPlain1);
             const uint32_t o0 = base + ((uint32_t)pay[b] << 2);
 #pragma unroll
             for (int r = 0; r < kMain; ++r) {
               const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
-              T0[r] += even_bytes_t(w);
-              T1[r] += odd_bytes_t(w);
+              Tw[r] += w;
+              To[r] += odd_bytes_t(w);
             }
             ++b;
           }
           // cells that k beams of the group share: one entry of weight k.  Two entries of equal weight are one pair: two loads
-          // added byte-wise (cell values <= 100), then one multiply-add per field; a weight without a partner is a single.
+          // added byte-wise (cell values <= 100), then one multiply-add per sum; a weight without a partner is a single.
           // (The host only builds weighted entries when the whole group's weight fits one flush.)
           for (int k = pe; k < se; k += 2) {
+            TILE_CN(kCnSingle);
             const uint32_t dm = *reinterpret_cast<const uint32_t *>(pay + k);
             const uint32_t o0 = base + ((dm & 0xFFFFu) << 2);
             const uint32_t kk = dm >> 16;
 #pragma unroll
             for (int r = 0; r < kMain; ++r) {
               const uint32_t w = lds_u32(o0 + r * 8 * pitchB);
-              T0[r] += even_bytes_t(w) * kk;
-              T1[r] += odd_bytes_t(w) * kk;
+              Tw[r] += w * kk;
+              To[r] += odd_bytes_t(w) * kk;
             }
           }
           for (int k = ps; k < pe2; k += 4) {
+            TILE_CN(kCnPair);
             const uint2 dp = *reinterpret_cast<const uint2 *>(pay + k);
             const uint32_t o0 = base + 4u * __byte_perm(dp.x, 0, 0x4410), o1 = base + 4u * __byte_perm(dp.x, 0, 0x4432);
             const uint32_t kk = dp.y;
@@ -538,49 +571,53 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
             for (int r = 0; r < kMain; ++r) {
               const uint32_t w = lds_u32(o0 + r * 8 * pitchB) +
                                  lds_u32(o1 + r * 8 * pitchB);
-              T0[r] += even_bytes_t(w) * kk;
-              T1[r] += odd_bytes_t(w) * kk;
+              Tw[r] += w * kk;
+              To[r] += odd_bytes_t(w) * kk;
             }
           }
           if (tail) {
             // the tail row nY - 1, lane-parallel over the entries: lane-row y_l reads entry y_l, y_l + 8, ... (its descriptor
             // with one LDS.U16 / LDS.32 / LDS.64 from 8 neighbouring entries, then the tail word of its column)
             const uint32_t tb = smem_u32(S8) + (uint32_t)(((nY - 1) * pitch_w + 4 * xt + j_l) * 4);
-            uint32_t t0 = 0, t1 = 0;
+            uint32_t tw = 0, to = 0;
             for (int k = b0 + y_l; k < pe; k += 8) {
+              TILE_CN(kCnTailPlain);
               const uint32_t w = lds_u32(tb + ((uint32_t)pay[k] << 2));
-              t0 += even_bytes_t(w);
-              t1 += odd_bytes_t(w);
+              tw += w;
+              to += odd_bytes_t(w);
             }
             for (int k = pe + 2 * y_l; k < se; k += 16) {
+              TILE_CN(kCnTailSingle);
               const uint32_t dm = *reinterpret_cast<const uint32_t *>(pay + k);
               const uint32_t w = lds_u32(tb + ((dm & 0xFFFFu) << 2));
-              t0 += even_bytes_t(w) * (dm >> 16);
-              t1 += odd_bytes_t(w) * (dm >> 16);
+              tw += w * (dm >> 16);
+              to += odd_bytes_t(w) * (dm >> 16);
             }
             for (int k = ps + 4 * y_l; k < pe2; k += 32) {
+              TILE_CN(kCnTailPair);
               const uint2 dp = *reinterpret_cast<const uint2 *>(pay + k);
               const uint32_t w = lds_u32(tb + 4u * __byte_perm(dp.x, 0, 0x4410)) + lds_u32(tb + 4u * __byte_perm(dp.x, 0, 0x4432));
-              t0 += even_bytes_t(w) * dp.y;
-              t1 += odd_bytes_t(w) * dp.y;
+              tw += w * dp.y;
+              to += odd_bytes_t(w) * dp.y;
             }
-            T0[kRowTiles - 1] = t0;
-            T1[kRowTiles - 1] = t1;
+            Tw[kRowTiles - 1] = tw;
+            To[kRowTiles - 1] = to;
           }
-          flush(T0, T1);
+          flush(Tw, To);
         }
         // EDGE beams of this group (window partly outside the grid): the same word loads with rows / words outside the
         // band allocation masked (they index outside [0, data_size) or wrap in the reference; the wrapped part is added
         // from the wrap2 list below).  Rows / words inside the allocation but beyond the valid cells are zero padding.
         while (eb < ee) {
           const int ce = min(ee, eb + kChunkBeams);
-          uint32_t T0[kRowTiles], T1[kRowTiles];
+          uint32_t Tw[kRowTiles], To[kRowTiles];
 #pragma unroll
-          for (int r = 0; r < kRowTiles; ++r) { T0[r] = 0; T1[r] = 0; }
+          for (int r = 0; r < kRowTiles; ++r) { Tw[r] = 0; To[r] = 0; }
           for (int b0 = eb; b0 < ce; b0 += 32) {
             const int cn = min(32, ce - b0);
             const int32_t mine = (lane < cn) ? f.edge[b0 + lane] : 0;
             for (int k = 0; k < cn; ++k) {
+              TILE_CN(kCnEdge);
               const int32_t ev = __shfl_sync(0xffffffffu, mine, k);
               const int rowb = (int)(int16_t)(ev & 0xFFFF), wq = (ev >> 16) + 4 * xt + j_l;
               const int row0 = rowb + ybase;
@@ -589,19 +626,19 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
               for (int r = 0; r < kMain; ++r) {
                 const int row = row0 + 8 * r;
                 const uint32_t w = (cv && (unsigned)row < (unsigned)f.alloc_rows) ? S[row * pitch_w + wq] : 0u;
-                T0[r] += even_bytes_t(w);
-                T1[r] += odd_bytes_t(w);
+                Tw[r] += w;
+                To[r] += odd_bytes_t(w);
               }
               if (tail) {   // the tail row in lane-row 0 only (the flush sums the lane-rows)
                 const int row = rowb + nY - 1;
                 const uint32_t w = (y_l == 0 && cv && (unsigned)row < (unsigned)f.alloc_rows) ? S[row * pitch_w + wq] : 0u;
-                T0[kRowTiles - 1] += even_bytes_t(w);
-                T1[kRowTiles - 1] += odd_bytes_t(w);
+                Tw[kRowTiles - 1] += w;
+                To[kRowTiles - 1] += odd_bytes_t(w);
               }
             }
           }
           eb = ce;
-          flush(T0, T1);
+          flush(Tw, To);
         }
        }
       }
@@ -862,6 +899,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_sweep_tile(SweepDev d, cons
   }
   if (pending_wait) cluster_wait();   // nobody leaves while a leader may still read its shared memory
   TILE_TM_END;
+  TILE_CN_END;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1414,5 +1452,21 @@ extern "C" int b200_tile_timers(unsigned long long * out, int reset)
     if (cudaMemcpyToSymbol(g_tile_timers, zero, sizeof(zero)) != cudaSuccess) return -1;
   }
   return kTmCount;
+}
+#endif
+
+#ifdef B200_TILE_COUNTS
+// loop-trip totals of the counting build, in the order of the kCn* enum: copied to out (when non-null), then zeroed when
+// reset != 0.  Returns the number of counters, or -1 on a CUDA error.
+extern "C" int b200_tile_counts(unsigned long long * out, int reset)
+{
+  using namespace b200;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  if (out && cudaMemcpyFromSymbol(out, g_tile_counts, sizeof(g_tile_counts)) != cudaSuccess) return -1;
+  if (reset) {
+    const unsigned long long zero[kCnCount] = {};
+    if (cudaMemcpyToSymbol(g_tile_counts, zero, sizeof(zero)) != cudaSuccess) return -1;
+  }
+  return kCnCount;
 }
 #endif
