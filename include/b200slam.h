@@ -183,6 +183,11 @@ int b200sm_batch_tile_layout(b200sm * h, int32_t layout[4]);
  * EDGE group (beams), (angle, phase, band, alignment) groups cut into more than one item, multi entries (cell, multiplicity),
  * largest multiplicity, largest plain group (beams), wrap2 entries}. */
 int b200sm_batch_tile_stats(b200sm * h, int32_t stats[8]);
+/* The tiled cluster kernel's plan for a geometry, without a handle or a device: in = {grid row stride, grid height, poses in x,
+ * poses in y, angles, beams per query, longest candidate scan (readings, rounded up to 4), penalised (1 / 0), pairs, SMs, forced
+ * cluster size, minimum angle chunks (0 = automatic), tail layout allowed (1 / 0)}; out = {refusal reason (0 = the kernel runs),
+ * cluster size, angle chunks, bands, rows per band, dynamic shared memory per CTA (bytes), tail row (1 / 0)}. */
+int b200sm_tile_plan(const int32_t in[13], int32_t out[7]);
 /* How the last fetch finished its pairs: stats = {pairs whose volume was all zero (all poses tie: closed form, once per
  * query; with use_response_expansion: pairs with an empty raster, closed form of the widest expansion pass), pairs handed one by one to the single-match path (tie list overflow with a non-zero best, response expansion),
  * pairs, 0}. */

@@ -120,6 +120,7 @@ def lib():
     L.b200sm_batch_tile_info.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_tile_stats.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_tile_layout.argtypes = [C.c_void_p, _IP]
+    L.b200sm_tile_plan.argtypes = [_IP, _IP]
     L.b200sm_batch_fetch_stats.argtypes = [C.c_void_p, _IP]
     L.b200sm_batch_upload_timing.argtypes = [C.c_void_p, _DP]
     L.b200sm_batch_reduce_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]

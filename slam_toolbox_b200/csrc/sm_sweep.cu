@@ -396,14 +396,12 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
   SweepHost & S = h->sweep;
   S.uploaded = S.ran = false;
   S.zero.done.clear(); S.zero_exp.done.clear();
-  // readouts of the kernel choice: the builder that succeeds fills in its own.  The builders' refusal codes (tile_info[5],
+  // readouts of the kernel choice: the builder that succeeds fills in its own.  The builders' refusal codes (tile_refusal,
   // fast_refusal) stay until that builder runs again.
   S.kernel = kSweepGeneric; S.refused_reason = 0;
   S.fast.enabled = 0; S.tile.enabled = 0;
   std::fill(S.beam_counts, S.beam_counts + 3, 0);
-  for (int i = 0; i < 8; ++i) if (i != 5) S.tile_info[i] = 0;
-  std::fill(S.tile_stats, S.tile_stats + 8, 0);
-  std::fill(S.tile_layout, S.tile_layout + 4, 0);
+  S.tile_plan = TilePlan{}; S.tile_clusters = 0; S.tile_stats = TileStats{};
   if (!queries || nq <= 0 || !scans || nscans <= 0 || !chain_start || nchains <= 0) {
     set_last_error("sweep: empty or NULL input");
     return B200_ERR_INVALID_ARG;
@@ -601,7 +599,7 @@ static int sweep_upload(b200sm * h, const b200_scan * queries, int nq, const b20
     if (h->sweep_kernel == 1 && build_fast_tables(h, S, st)) S.kernel = kSweepFast;
     else if (build_tile_tables(h, S, st)) S.kernel = kSweepTile;
     else if (h->sweep_kernel != 1 && build_fast_tables(h, S, st)) S.kernel = kSweepFast;
-    else S.refused_reason = S.tile_info[5] ? 100 + S.tile_info[5] : S.fast_refusal;
+    else S.refused_reason = S.tile_refusal ? 100 + S.tile_refusal : S.fast_refusal;
   }
   const auto t_tab1 = std::chrono::steady_clock::now();
   auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
@@ -991,7 +989,7 @@ int b200sm_batch_info(b200sm * h, int32_t info[8])
   info[0] = S.kernel;
   for (int i = 0; i < 3; ++i) info[1 + i] = S.beam_counts[i];
   info[4] = S.refused_reason;
-  info[5] = S.kernel == kSweepTile ? S.tile_grid : (S.kernel == kSweepFast ? S.fast_blocks : S.blocks);
+  info[5] = S.kernel == kSweepTile ? S.tile_clusters * S.tile_plan.C : (S.kernel == kSweepFast ? S.fast_blocks : S.blocks);
   info[6] = S.npairs; info[7] = S.nitems;
   return B200_OK;
 }
@@ -999,21 +997,39 @@ int b200sm_batch_info(b200sm * h, int32_t info[8])
 int b200sm_batch_tile_info(b200sm * h, int32_t info[8])
 {
   if (!h || !info || !h->sweep.uploaded) return B200_ERR_INVALID_ARG;
-  for (int i = 0; i < 8; ++i) info[i] = h->sweep.tile_info[i];
+  const SweepHost & S = h->sweep;
+  const TilePlan & p = S.tile_plan;
+  info[0] = S.tile.enabled; info[1] = p.C; info[2] = p.V; info[3] = p.nbands; info[4] = p.band_rows; info[5] = S.tile_refusal;
+  info[6] = S.tile_clusters; info[7] = (int32_t)(p.smem / 1024);
   return B200_OK;
 }
 
 int b200sm_batch_tile_layout(b200sm * h, int32_t layout[4])
 {
   if (!h || !layout || !h->sweep.uploaded) return B200_ERR_INVALID_ARG;
-  for (int i = 0; i < 4; ++i) layout[i] = h->sweep.tile_layout[i];
+  const TilePlan & p = h->sweep.tile_plan;
+  layout[0] = p.ytile_rows; layout[1] = p.ytiles; layout[2] = p.xtiles; layout[3] = p.tail;
   return B200_OK;
 }
 
 int b200sm_batch_tile_stats(b200sm * h, int32_t stats[8])
 {
   if (!h || !stats || !h->sweep.uploaded) return B200_ERR_INVALID_ARG;
-  for (int i = 0; i < 8; ++i) stats[i] = h->sweep.tile_stats[i];
+  static_assert(sizeof(TileStats) == 8 * sizeof(int32_t), "TileStats holds the 8 stats in their ABI order");
+  std::memcpy(stats, &h->sweep.tile_stats, sizeof(TileStats));
+  return B200_OK;
+}
+
+int b200sm_tile_plan(const int32_t in[13], int32_t out[7])
+{
+  if (!in || !out) return B200_ERR_INVALID_ARG;
+  // the grid, window, beams, batch and SMs positive (max_n, do_penalize, cluster, chunks and tail may be 0); the window small
+  // enough that the planner's byte counts stay in int
+  for (int i = 0; i < 13; ++i)
+    if (in[i] < (i == 6 || i == 7 || i >= 10 ? 0 : 1) || in[i] > (i == 2 || i == 3 ? 2048 : 1 << 20)) return B200_ERR_INVALID_ARG;
+  const TilePlan p = plan_tile(TilePlanIn{in[0], in[1], in[2], in[3], in[4], in[5], in[6], in[7], in[8], in[9], in[10], in[11], in[12]});
+  const int32_t v[7] = {p.refused, p.C, p.V, p.nbands, p.band_rows, (int32_t)p.smem, p.tail};
+  std::copy(v, v + 7, out);
   return B200_OK;
 }
 

@@ -1091,70 +1091,58 @@ int parity_refusal(const GridGeom & g, const std::vector<CorrPlan> & plans)
   return 0;
 }
 
-bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
+// Refusals (the sweep then runs on the generic kernel, which takes any n and nA): plan_tile's 2, 4, 9 (more x- / y-tiles than the
+// item record holds) and 5 (the plan's shared memory exceeds 227 KB), schedule_query's 8 and 10 to 13.  Packed fields and bounds:
+//   TileSeq.a0 / chunk (int16)   nA <= 4096                                                  -> 2
+//   item al (6 bits)             nAc <= 63 angles per chunk (the V loop)                     -> 4 when no V fits
+//   item plain count (10 bits)   pieces of <= kChunkBeams = 640 beams
+//   item singles (6 bits)        weighted entries only in groups of <= kChunkBeams beams: one single per distinct weight
+//                                k >= 2 (2 + 3 + ... + 36 = 665 > 640: <= 34 weights) + the odd plain beam: <= 35; without
+//                                pairing (B200_TILE_PAIRS=0) the encoder returns singles beyond 62 to the plain list
+//   item pairs (8 bits)          a pair weighs >= 4 beams: <= 640 / 4 = 160 per group
+//   (all three, and pb, are checked per record by build_block_items)                        -> 13
+//   one angle's block            payload <= n + 32 entries, records per the one_angle minimum  -> 8
+//   TileSeq.nitems (int16)       records of one block                                        -> 10
+//   item pb / pe (16 bits)       payload entries of one block                                -> 11
+//   TileSeq.off (int32)          descriptor blob bytes                                       -> 12
+//   cell-list staging            max_n > 4096: the raster reads the cells from global memory    (no refusal needed)
+TilePlan plan_tile(const TilePlanIn & in)
 {
-  const GridGeom & g = h->g;
-  const CorrPlan & p0 = S.plans[0];
-  const int nX = p0.nX, nY = p0.nY, nA = p0.nA, n = p0.n, nq = S.nq, P = nX * nY;
-  TileDev & T = S.tile;
-  T = TileDev{};
-  auto bail = [&](int why) {
-    for (int i = 0; i < 8; ++i) S.tile_stats[i] = 0;
-    S.tile_info[5] = why;
-    return false;
-  };
-  // Packed fields and their bounds (a refusal runs the sweep on the generic kernel, which takes any n and nA):
-  //   TileSeq.a0 / chunk (int16)   nA <= 4096                                                  -> 2
-  //   item al (6 bits)             nAc <= 63 angles per chunk (the V loop)                     -> 4 when no V fits
-  //   item plain count (10 bits)   pieces of <= kChunkBeams = 640 beams
-  //   item singles (6 bits)        weighted entries only in groups of <= kChunkBeams beams: one single per distinct weight
-  //                                k >= 2 (2 + 3 + ... + 36 = 665 > 640: <= 34 weights) + the odd plain beam: <= 35; without
-  //                                pairing (B200_TILE_PAIRS=0) the encoder returns singles beyond 62 to the plain list
-  //   item pairs (8 bits)          a pair weighs >= 4 beams: <= 640 / 4 = 160 per group
-  //   (all three, and pb, are checked per record by build_block_items)                        -> 13
-  //   one angle's block            payload <= n + 32 entries, records per the one_angle minimum  -> 8
-  //   TileSeq.nitems (int16)       records of one block                                        -> 10
-  //   item pb / pe (16 bits)       payload entries of one block                                -> 11
-  //   TileSeq.off (int32)          descriptor blob bytes                                       -> 12
-  //   cell-list staging            max_n > 4096: the raster reads the cells from global memory    (no refusal needed)
-  if (const int why = parity_refusal(g, S.plans)) return bail(why);
-  if ((g.stride & 1) || nA < 1 || nA > 4096) return bail(2);
+  auto refuse = [](int why) { TilePlan r; r.refused = why; return r; };
+  const int nX = in.nX, nY = in.nY, nA = in.nA, n = in.n, P = nX * nY;
+  if ((in.stride & 1) || nA < 1 || nA > 4096) return refuse(2);
   // ---- geometry of one parity sub-grid ----
-  int pitch_w = (g.stride / 2 + 16 + 3) / 4;             // sub-grid row + the 3-word overhang of the last x-tile
+  int pitch_w = (in.stride / 2 + 16 + 3) / 4;            // sub-grid row + the 3-word overhang of the last x-tile
   while ((pitch_w & 7) != 4) ++pitch_w;                  // 8 rows x 4 words of a warp hit 32 distinct banks
   // y-tile layout, by the row-tile loads of one beam and x-tile (in eighths of a row tile): 48-row y-tiles of six row tiles, or
   // 40-row y-tiles of five + the tail row (one descriptor and one word load per 8 entries, i.e. 2 / 8).  41 rows: 42 vs 48; 81
   // rows: 82 vs 96; 45 rows: 82 vs 48 (stays on 48-row tiles)
   const int yt48 = (nY + 47) / 48, yt40 = std::max(1, (nY - 1 + 39) / 40);
-  // B200_TILE_TAIL=0 / B200_TILE_PAIRS=0 switch the tail layout / the weight-2 entries and pairing off, to measure each part alone
-  const bool tail = env_int("B200_TILE_TAIL", 1) != 0 && 8 * 5 * yt40 + 2 < 8 * 6 * yt48;
-  const bool pairs_on = env_int("B200_TILE_PAIRS", 1) != 0;
+  const bool tail = in.tail && 8 * 5 * yt40 + 2 < 8 * 6 * yt48;
   const int ytile_rows = tail ? 40 : 48;
   const int xtiles = (nX + 3 + 15) / 16, ytiles = tail ? yt40 : yt48;
-  if (xtiles > kItemMaxXTiles || ytiles > kItemMaxYTiles) return bail(9);
-  const int rows_valid = (g.height + 1) / 2;
+  if (xtiles > kItemMaxXTiles || ytiles > kItemMaxYTiles) return refuse(9);
+  const int rows_valid = (in.height + 1) / 2;
   const int halo = nY + 2;                               // rows a beam window reaches below its base row (idle row tiles are clamped) + the wrapped row
   const int base_rows = std::max(1, rows_valid - nY + 1);   // distinct base rows of beams whose window is inside the grid
   // ---- choose the number of angle chunks V and of bands ----
-  const int sms = h->sms;
-  int want_c = h->tile_cluster > 0 ? h->tile_cluster : env_int("B200_SWEEP_CLUSTER", 0);
+  int want_c = in.cluster;
   if (want_c <= 0) {
     // throughput mode (one CTA per pair) once the batch fills the GPU, otherwise spread a pair over a cluster
     want_c = 1;
-    while (want_c < kTileMaxCluster && S.npairs * want_c * 2 <= sms) want_c *= 2;
+    while (want_c < kTileMaxCluster && in.npairs * want_c * 2 <= in.sms) want_c *= 2;
   }
   int Cc = 1;
   while (Cc * 2 <= std::min(want_c, kTileMaxCluster)) Cc *= 2;
   Cc = std::min(Cc, nA);
   while (Cc & (Cc - 1)) --Cc;
   const int budget = 227 * 1024 - (int)sizeof(TileShared) - 256;
-  const int int_ties = (!S.do_penalize && (double)n * kOccupied < 0.9e6) ? 1 : 0;
+  const int int_ties = (!in.do_penalize && (double)n * kOccupied < 0.9e6) ? 1 : 0;
   const int probs_bytes = (P * (int_ties ? 4 : 8) + 15) & ~15;   // per-cell maximum image: integer sums or FP64 responses
-  int force_v = h->tile_chunks > 0 ? h->tile_chunks : env_int("B200_SWEEP_CHUNKS", 0);
   int bestV = 0, bestNb = 0, bestB = 0, bestStage = 0;
   long bestCost = -1;
   for (int V = Cc; V <= nA; ++V) {
-    if (force_v > 0 && V < std::min(force_v, nA)) continue;   // "sweep_chunks" = at least this many chunks
+    if (in.chunks > 0 && V < std::min(in.chunks, nA)) continue;   // "sweep_chunks" = at least this many chunks
     const int nAc = (nA + V - 1) / V;
     if ((nA + nAc - 1) / nAc != V || nAc > 63) continue;   // same chunk size as a smaller V; group ids are bytes
     const int a_bytes = (4 * (kAGuardLo + nAc * P + kAGuardHi) + 15) & ~15;
@@ -1188,251 +1176,288 @@ bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
     const long cost = (long)((V + Cc - 1) / Cc) * (nbv * w_raster + nAc * w_angle);
     if (bestCost < 0 || cost < bestCost) { bestCost = cost; bestV = V; bestNb = nbv; bestB = B; bestStage = stage; }
   }
-  if (bestCost < 0) return bail(4);
-  const int V = bestV, nbands = bestNb, B = bestB, nAc = (nA + V - 1) / V, stage_bytes = bestStage;
-  const int C = std::min(Cc, V);
-  int alloc_rows = std::min(B + halo, rows_valid + halo - nY);
-  alloc_rows = std::max(alloc_rows, 1);
-  const size_t s_bytes = ((size_t)alloc_rows * pitch_w * 4 + 15) & ~(size_t)15;
-  const size_t a_bytes = (4 * ((size_t)kAGuardLo + (size_t)nAc * P + kAGuardHi) + 15) & ~(size_t)15;   // A and its guard words
-  T.C = C; T.V = V; T.nAc = nAc; T.nbands = nbands; T.band_rows = B; T.alloc_rows = alloc_rows; T.pitch_w = pitch_w;
-  T.xtiles = xtiles; T.ytiles = ytiles; T.tail = tail ? 1 : 0; T.stage_bytes = stage_bytes;
-  T.int_ties = int_ties;
-  {
-    // distinct non-zero smear values, ascending; up to 4 -> levelled (atomic-free) raster
-    std::vector<uint8_t> lv(g.kernel.begin(), g.kernel.end());
-    std::sort(lv.begin(), lv.end());
-    lv.erase(std::unique(lv.begin(), lv.end()), lv.end());
-    if (!lv.empty() && lv[0] == 0) lv.erase(lv.begin());
-    T.nlevels = (!lv.empty() && lv.size() <= 4) ? (int)lv.size() : 0;
-    for (int i = 0; i < 4; ++i) T.level[i] = i < T.nlevels ? lv[i] : 0;
-    // the levelled raster's tap masks: for level l and class c = 2 ky0 + kx0 (the first kernel row / column of a point's phase
-    // parity), bit 8 dy + dx for the tap ky = ky0 + 2 dy, kx = kx0 + 2 dx of that value
-    const int ks = g.ksize;
-    T.tap_masks = (T.nlevels > 0 && ks <= kTileMaxMaskKsize) ? 1 : 0;
-    if (T.tap_masks)
-      for (int l = 0; l < T.nlevels; ++l)
-        for (int c = 0; c < 4; ++c)
-          for (int ky = c >> 1; ky < ks; ky += 2)
-            for (int kx = c & 1; kx < ks; kx += 2)
-              if (g.kernel[(size_t)ky * ks + kx] == T.level[l]) T.tap_mask[l][c] |= 1ull << (8 * (ky >> 1) + (kx >> 1));
-  }
-  T.off_A = s_bytes + 4 * kAGuardLo; T.off_probs = s_bytes + a_bytes; T.off_stage = (T.off_probs + probs_bytes + 127) & ~(size_t)127;
-  T.off_cells = T.off_stage + 2 * (size_t)stage_bytes;
+  if (bestCost < 0) return refuse(4);
+  TilePlan p;
+  p.C = std::min(Cc, bestV); p.V = bestV; p.nAc = (nA + bestV - 1) / bestV; p.nbands = bestNb; p.band_rows = bestB;
+  p.alloc_rows = std::max(std::min(bestB + halo, rows_valid + halo - nY), 1); p.pitch_w = pitch_w; p.xtiles = xtiles;
+  p.ytiles = ytiles; p.ytile_rows = ytile_rows; p.tail = tail ? 1 : 0; p.stage_bytes = bestStage; p.int_ties = int_ties;
+  const size_t s_bytes = ((size_t)p.alloc_rows * pitch_w * 4 + 15) & ~(size_t)15;
+  const size_t a_bytes = (4 * ((size_t)kAGuardLo + (size_t)p.nAc * P + kAGuardHi) + 15) & ~(size_t)15;   // A and its guard words
+  p.off_A = s_bytes + 4 * kAGuardLo; p.off_probs = s_bytes + a_bytes; p.off_stage = (p.off_probs + probs_bytes + 127) & ~(size_t)127;
+  p.off_cells = p.off_stage + 2 * (size_t)p.stage_bytes;
   // cell-list staging only where the chosen plan leaves room for it (it must not cost a band or a chunk)
-  int cell_cap = d_max_n_ok(S.max_n) ? S.max_n : 0;                     // entries per cell staging buffer (0 = read cells from global)
-  if (T.off_cells + 2 * (size_t)cell_cap * 4 + sizeof(TileShared) + 64 > 227 * 1024) cell_cap = 0;
-  T.cell_cap = cell_cap;
-  size_t smem = T.off_cells + 2 * (size_t)cell_cap * 4;
+  int cell_cap = d_max_n_ok(in.max_n) ? in.max_n : 0;                   // entries per cell staging buffer (0 = read cells from global)
+  if (p.off_cells + 2 * (size_t)cell_cap * 4 + sizeof(TileShared) + 64 > 227 * 1024) cell_cap = 0;
+  p.cell_cap = cell_cap;
+  size_t smem = p.off_cells + 2 * (size_t)cell_cap * 4;
   // idle lanes of the last y-tile read up to (ytile_rows * ytiles - nY) rows past the band (see the kernel): keep those reads inside
   // the allocation even when everything behind S is small (tiny search windows)
   const size_t overrun = (size_t)std::max(ytile_rows * ytiles - nY + 1, 1) * pitch_w * 4;
   if (smem - s_bytes < overrun) smem = s_bytes + overrun;
-  if (smem + sizeof(TileShared) + 64 > 227 * 1024) return bail(5);
+  if (smem + sizeof(TileShared) + 64 > 227 * 1024) return refuse(5);
+  p.smem = smem;
+  return p;
+}
 
-  // ---- per-query descriptor blocks and schedules ----
-  const int nstage = 4 * nbands;
-  std::vector<uint8_t> blob;
-  std::vector<TileSeq> seq;
-  std::vector<int32_t> seq_start((size_t)nq * C + 1, 0);
-  BeamLists lists;
-  std::vector<BeamClasses> cls(nA);
-  blob.reserve((size_t)nq * nA * n * 2 + 4096);
-  struct Encoded { int32_t tbl[16]; std::vector<uint16_t> pay; };
-  std::vector<Encoded> enc((size_t)nA * nstage);
-  for (int q = 0; q < nq; ++q) {
-    const CorrPlan & pl = S.plans[q];
-    // one host-pool task per angle: classify its beams, then sort / run-length encode its groups stage by stage
-    auto one_angle = [&](int a) {
-      classify_beams(g, pl, a, pitch_w, B, nbands, cls[a]);
-      // the angle's groups of every stage: table of (plain begin, singles begin, pairs begin, pairs end) per alignment, relative
-      // to the angle's own payload (whose start is 4-entry aligned in the block), and the payload
-      for (int sg = 0; sg < nstage; ++sg) {
-        Encoded & E = enc[(size_t)a * nstage + sg];
-        std::vector<uint16_t> & pay = E.pay;
-        pay.clear();
-        for (int m = 0; m < 4; ++m) {
-          std::vector<uint16_t> & gk = cls[a].fast[sg * 4 + m];
-          std::sort(gk.begin(), gk.end());
-          while (pay.size() & 3) pay.push_back(0);   // the plain list is read with 64-bit loads
-          const int pb = (int)pay.size();
-          // run-length encode: beams that land in the same cell share one entry of weight k (one load per row, fields times
-          // k), provided the whole group fits one flush.  Entries of equal weight are then paired (two loads added byte-wise,
-          // one multiply per field); weight-1 beams stay in the plain list.
-          std::vector<std::pair<uint16_t, uint16_t>> multi;   // (offset, weight), by ascending weight
-          encode_runs(gk, pairs_on ? 2 : 3, !h->no_dedup && gk.size() <= (size_t)kChunkBeams, pay, multi);
-          std::stable_sort(multi.begin(), multi.end(),
-                           [](const std::pair<uint16_t, uint16_t> & x, const std::pair<uint16_t, uint16_t> & y) { return x.second < y.second; });
-          std::vector<std::pair<uint16_t, uint16_t>> single;   // (offset, weight)
-          std::vector<uint16_t> pairs;                         // offset, offset, weight, 0
-          for (size_t i = 0; i < multi.size();) {
-            if (pairs_on && i + 1 < multi.size() && multi[i + 1].second == multi[i].second) {
-              pairs.insert(pairs.end(), {multi[i].first, multi[i + 1].first, multi[i].second, (uint16_t)0});
-              i += 2;
-            } else {
-              single.push_back(multi[i]);
-              i += 1;
-            }
-          }
-          // the item record counts the singles in 6 bits.  With pairing there are at most 35 (see the field bounds); without it
-          // (B200_TILE_PAIRS=0) every merged cell is a single: those beyond kMaxSingles - 1 (one slot stays free for the odd plain
-          // beam below) go back to the plain list as k plain beams each
-          while (single.size() > (size_t)kMaxSingles - 1) {
-            for (uint16_t t = 0; t < single.back().second; ++t) pay.push_back(single.back().first);
-            single.pop_back();
-          }
-          // the tail row reads entries 8 apart in each lane-row: spread the plain list's neighbouring (sorted, so nearby)
-          // word offsets over the lane-rows so that their 4-word runs rarely share banks (48-row y-tiles have no tail row)
-          if (tail) spread_rows(pay.begin() + pb, pay.end());
-          // the singles (offset, weight; read as 32-bit words) start where the plain list ends: keep that index even by
-          // moving an odd plain list's last entry into the singles with weight 1
-          if (((int)pay.size() - pb) & 1) {
-            const uint16_t last = pay.back();
-            pay.pop_back();
-            single.emplace_back(last, (uint16_t)1);
-          }
-          const int sb = (int)pay.size();
-          for (auto & s1 : single) { pay.push_back(s1.first); pay.push_back(s1.second); }
-          const int se = (int)pay.size();
-          if (!pairs.empty()) while (pay.size() & 3) pay.push_back(0);   // the pairs are read as 64-bit words
-          pay.insert(pay.end(), pairs.begin(), pairs.end());
-          E.tbl[4 * m + 0] = pb; E.tbl[4 * m + 1] = sb; E.tbl[4 * m + 2] = se; E.tbl[4 * m + 3] = (int)pay.size();
+// The levelled raster's smear levels: the kernel's distinct non-zero values, ascending, when there are at most 4 (else none: the
+// raster takes the atomic path), and their tap masks: for level l and class c = 2 ky0 + kx0 (the first kernel row / column of a
+// point's phase parity), bit 8 dy + dx for the tap ky = ky0 + 2 dy, kx = kx0 + 2 dx of that value
+static void raster_levels(const std::vector<uint8_t> & kernel, int ks, TileDev & T)
+{
+  std::vector<uint8_t> lv(kernel.begin(), kernel.end());
+  std::sort(lv.begin(), lv.end());
+  lv.erase(std::unique(lv.begin(), lv.end()), lv.end());
+  if (!lv.empty() && lv[0] == 0) lv.erase(lv.begin());
+  T.nlevels = (!lv.empty() && lv.size() <= 4) ? (int)lv.size() : 0;
+  for (int i = 0; i < 4; ++i) T.level[i] = i < T.nlevels ? lv[i] : 0;
+  T.tap_masks = (T.nlevels > 0 && ks <= kTileMaxMaskKsize) ? 1 : 0;
+  if (T.tap_masks)
+    for (int l = 0; l < T.nlevels; ++l)
+      for (int c = 0; c < 4; ++c)
+        for (int ky = c >> 1; ky < ks; ky += 2)
+          for (int kx = c & 1; kx < ks; kx += 2)
+            if (kernel[(size_t)ky * ks + kx] == T.level[l]) T.tap_mask[l][c] |= 1ull << (8 * (ky >> 1) + (kx >> 1));
+}
+
+// One angle's groups of one stage: table of (plain begin, singles begin, singles end, pairs end) per alignment, relative to the
+// angle's own payload (whose start is 4-entry aligned in the block), and the payload
+struct Encoded { int32_t tbl[16]; std::vector<uint16_t> pay; };
+
+// Classifies the beams of angle a of plan pl into c, then sorts and run-length encodes its FAST groups stage by stage into
+// enc[0 .. 4 nbands).  p.tail spreads the plain lists over the lane-rows of the tail row; pairs_on pairs entries of equal weight and
+// merges runs of 2 (else of 3); no_dedup keeps one entry per beam.
+static void encode_angle(const GridGeom & g, const CorrPlan & pl, int a, const TilePlan & p, bool pairs_on, bool no_dedup, BeamClasses & c,
+                         Encoded * enc)
+{
+  classify_beams(g, pl, a, p.pitch_w, p.band_rows, p.nbands, c);
+  for (int sg = 0; sg < 4 * p.nbands; ++sg) {
+    Encoded & E = enc[sg];
+    std::vector<uint16_t> & pay = E.pay;
+    pay.clear();
+    for (int m = 0; m < 4; ++m) {
+      std::vector<uint16_t> & gk = c.fast[sg * 4 + m];
+      std::sort(gk.begin(), gk.end());
+      while (pay.size() & 3) pay.push_back(0);   // the plain list is read with 64-bit loads
+      const int pb = (int)pay.size();
+      // run-length encode: beams that land in the same cell share one entry of weight k (one load per row, fields times
+      // k), provided the whole group fits one flush.  Entries of equal weight are then paired (two loads added byte-wise,
+      // one multiply per field); weight-1 beams stay in the plain list.
+      std::vector<std::pair<uint16_t, uint16_t>> multi;   // (offset, weight), by ascending weight
+      encode_runs(gk, pairs_on ? 2 : 3, !no_dedup && gk.size() <= (size_t)kChunkBeams, pay, multi);
+      std::stable_sort(multi.begin(), multi.end(),
+                       [](const std::pair<uint16_t, uint16_t> & x, const std::pair<uint16_t, uint16_t> & y) { return x.second < y.second; });
+      std::vector<std::pair<uint16_t, uint16_t>> single;   // (offset, weight)
+      std::vector<uint16_t> pairs;                         // offset, offset, weight, 0
+      for (size_t i = 0; i < multi.size();) {
+        if (pairs_on && i + 1 < multi.size() && multi[i + 1].second == multi[i].second) {
+          pairs.insert(pairs.end(), {multi[i].first, multi[i + 1].first, multi[i].second, (uint16_t)0});
+          i += 2;
+        } else {
+          single.push_back(multi[i]);
+          i += 1;
         }
-        while (pay.size() & 3) pay.push_back(0);
       }
-    };
-    host_parallel_for(nA, one_angle);
-    append_beam_lists(cls, nstage, lists);
-    std::vector<uint16_t> pay;
-    std::vector<int32_t> tbl;
-    std::vector<int> nedge;
-    std::vector<uint2> items;
-    for (int r = 0; r < C; ++r) {
-      seq_start[(size_t)q * C + r] = (int32_t)seq.size();
-      for (int v = r; v < V; v += C) {
-        const int ca0 = v * nAc, cna = std::min(nAc, nA - ca0);
-        // the CTA's chunks alternate the stage order (phase 0 -> 3, then 3 -> 0, ...): each chunk starts on the (phase, band) the
-        // one before it ended on, whose sub-grid is still resident
-        const bool backward = ((v - r) / C) & 1, keep = v != r;
-        for (int si = 0; si < nstage; ++si) {
-          const int sg = backward ? nstage - 1 - si : si;
-          // sub-blocks: as many angles as fit one staging buffer
-          int a = ca0;
-          bool first_sub = true;
-          do {
-            tbl.clear(); pay.clear();
-            int na = 0, npieces = 0;   // pieces of the block's groups so far (items = pieces x tiles)
-            while (a + na < ca0 + cna) {
-              const Encoded & E = enc[(size_t)(a + na) * nstage + sg];
-              int ep = 0;
-              for (int m = 0; m < 4; ++m) ep += std::max(1, (E.tbl[4 * m + 1] - E.tbl[4 * m] + kChunkBeams - 1) / kChunkBeams);
-              const size_t hdr = (((size_t)(npieces + ep) * xtiles * ytiles * 8) + 15) & ~(size_t)15;
-              const size_t bytes = (hdr + (pay.size() + E.pay.size()) * 2 + 15) & ~(size_t)15;
-              const bool wide = pay.size() + E.pay.size() > 65535;   // item records hold 16-bit payload indices (pb, pe)
-              if (bytes > (size_t)stage_bytes || wide) {
-                if (na > 0) break;
-                return bail(wide ? 11 : 8);   // one angle does not fit the 16-bit indices / the staging buffer
-              }
-              const int shift = (int)pay.size();
-              for (int k = 0; k < 16; ++k) tbl.push_back(E.tbl[k] + shift);
-              pay.insert(pay.end(), E.pay.begin(), E.pay.end());
-              npieces += ep;
-              ++na;
-            }
-            nedge.assign((size_t)na * 4, 0);
-            for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)cls[a + (g2 >> 2)].edge[sg * 4 + (g2 & 3)].size();
-            if (!build_block_items(tbl, nedge, na, xtiles, ytiles, items)) return bail(13);
-            if (items.size() > 32767) return bail(10);   // TileSeq.nitems is 16-bit
-            int32_t * ts = S.tile_stats;
-            ts[0] += 1;
-            ts[1] += first_sub ? 0 : 1;
-            for (int g2 = 0; g2 < na * 4; ++g2) {
-              const int pb = tbl[4 * g2], mb = tbl[4 * g2 + 1], se = tbl[4 * g2 + 2], pe2 = tbl[4 * g2 + 3];
-              const int ps = pe2 > se ? ((se + 3) & ~3) : se;
-              ts[2] = std::max(ts[2], nedge[g2]);
-              ts[3] += mb - pb > kChunkBeams ? 1 : 0;
-              ts[4] += (se - mb) / 2 + (pe2 - ps) / 2;   // weighted entries: singles + both entries of every pair
-              for (int k = mb; k < se; k += 2) ts[5] = std::max(ts[5], (int32_t)pay[k + 1]);
-              for (int k = ps; k < pe2; k += 4) ts[5] = std::max(ts[5], (int32_t)pay[k + 2]);
-              ts[6] = std::max(ts[6], mb - pb);
-            }
-            const size_t hdr = ((items.size() * 8) + 15) & ~(size_t)15;
-            const size_t bytes = std::max<size_t>(16, (hdr + pay.size() * 2 + 15) & ~(size_t)15);
-            if (blob.size() + bytes > 0x7FFFFFF0u) return bail(12);   // TileSeq.off is a 32-bit byte offset
-            TileSeq e{};
-            e.off = (int32_t)blob.size();
-            e.bytes = (int32_t)bytes;
-            e.chunk = (int16_t)v; e.stage = (int16_t)sg; e.a0 = (int16_t)a; e.nitems = (int16_t)items.size();
-            e.flags = (first_sub ? kSeqNewStage : 0u) | ((first_sub && si == 0) ? kSeqNewChunk : 0u) |
-                      ((first_sub && si == 0 && keep) ? kSeqKeepGrid : 0u);
-            if (first_sub)
-              for (int aa = ca0; aa < ca0 + cna; ++aa)
-                if (!cls[aa].wrap2[sg].empty()) e.flags |= kSeqHasWrap;
-            blob.resize(blob.size() + bytes, 0);
-            if (!items.empty()) std::memcpy(blob.data() + e.off, items.data(), items.size() * 8);
-            if (!pay.empty()) std::memcpy(blob.data() + e.off + hdr, pay.data(), pay.size() * 2);
-            seq.push_back(e);
-            a += na;
-            first_sub = false;
-          } while (a < ca0 + cna);
-        }
-        seq.back().flags |= kSeqEndChunk;
+      // the item record counts the singles in 6 bits.  With pairing there are at most 35 (see the field bounds); without it
+      // (B200_TILE_PAIRS=0) every merged cell is a single: those beyond kMaxSingles - 1 (one slot stays free for the odd plain
+      // beam below) go back to the plain list as k plain beams each
+      while (single.size() > (size_t)kMaxSingles - 1) {
+        for (uint16_t t = 0; t < single.back().second; ++t) pay.push_back(single.back().first);
+        single.pop_back();
       }
+      // the tail row reads entries 8 apart in each lane-row: spread the plain list's neighbouring (sorted, so nearby)
+      // word offsets over the lane-rows so that their 4-word runs rarely share banks (48-row y-tiles have no tail row)
+      if (p.tail) spread_rows(pay.begin() + pb, pay.end());
+      // the singles (offset, weight; read as 32-bit words) start where the plain list ends: keep that index even by
+      // moving an odd plain list's last entry into the singles with weight 1
+      if (((int)pay.size() - pb) & 1) {
+        const uint16_t last = pay.back();
+        pay.pop_back();
+        single.emplace_back(last, (uint16_t)1);
+      }
+      const int sb = (int)pay.size();
+      for (auto & s1 : single) { pay.push_back(s1.first); pay.push_back(s1.second); }
+      const int se = (int)pay.size();
+      if (!pairs.empty()) while (pay.size() & 3) pay.push_back(0);   // the pairs are read as 64-bit words
+      pay.insert(pay.end(), pairs.begin(), pairs.end());
+      E.tbl[4 * m + 0] = pb; E.tbl[4 * m + 1] = sb; E.tbl[4 * m + 2] = se; E.tbl[4 * m + 3] = (int)pay.size();
+    }
+    while (pay.size() & 3) pay.push_back(0);
+  }
+}
+
+// The descriptor blocks of one query (its angles' classes cls and encodings enc, nstage per angle) and the schedule of each CTA r
+// of its cluster: the chunks r, r + C, ..., each stage of a chunk cut into sub-blocks of as many angles as fit one staging buffer.
+// Appends the blocks to blob, their records to seq and each CTA's first record to seq_start, adds to ts, and returns 0 or a
+// refusal code (8, 10 to 13).
+static int schedule_query(const TilePlan & p, int nA, const std::vector<BeamClasses> & cls, const std::vector<Encoded> & enc,
+                          std::vector<uint8_t> & blob, std::vector<TileSeq> & seq, std::vector<int32_t> & seq_start, TileStats & ts)
+{
+  const int C = p.C, nAc = p.nAc, nstage = 4 * p.nbands, xtiles = p.xtiles, ytiles = p.ytiles;
+  std::vector<uint16_t> pay;
+  std::vector<int32_t> tbl;
+  std::vector<int> nedge;
+  std::vector<uint2> items;
+  for (int r = 0; r < C; ++r) {
+    seq_start.push_back((int32_t)seq.size());
+    for (int v = r; v < p.V; v += C) {
+      const int ca0 = v * nAc, cna = std::min(nAc, nA - ca0);
+      // the CTA's chunks alternate the stage order (phase 0 -> 3, then 3 -> 0, ...): each chunk starts on the (phase, band) the
+      // one before it ended on, whose sub-grid is still resident
+      const bool backward = ((v - r) / C) & 1, keep = v != r;
+      for (int si = 0; si < nstage; ++si) {
+        const int sg = backward ? nstage - 1 - si : si;
+        // sub-blocks: as many angles as fit one staging buffer
+        int a = ca0;
+        bool first_sub = true;
+        do {
+          tbl.clear(); pay.clear();
+          int na = 0, npieces = 0;   // pieces of the block's groups so far (items = pieces x tiles)
+          while (a + na < ca0 + cna) {
+            const Encoded & E = enc[(size_t)(a + na) * nstage + sg];
+            int ep = 0;
+            for (int m = 0; m < 4; ++m) ep += std::max(1, (E.tbl[4 * m + 1] - E.tbl[4 * m] + kChunkBeams - 1) / kChunkBeams);
+            const size_t hdr = (((size_t)(npieces + ep) * xtiles * ytiles * 8) + 15) & ~(size_t)15;
+            const size_t bytes = (hdr + (pay.size() + E.pay.size()) * 2 + 15) & ~(size_t)15;
+            const bool wide = pay.size() + E.pay.size() > 65535;   // item records hold 16-bit payload indices (pb, pe)
+            if (bytes > (size_t)p.stage_bytes || wide) {
+              if (na > 0) break;
+              return wide ? 11 : 8;   // one angle does not fit the 16-bit indices / the staging buffer
+            }
+            const int shift = (int)pay.size();
+            for (int k = 0; k < 16; ++k) tbl.push_back(E.tbl[k] + shift);
+            pay.insert(pay.end(), E.pay.begin(), E.pay.end());
+            npieces += ep;
+            ++na;
+          }
+          nedge.assign((size_t)na * 4, 0);
+          for (int g2 = 0; g2 < na * 4; ++g2) nedge[g2] = (int)cls[a + (g2 >> 2)].edge[sg * 4 + (g2 & 3)].size();
+          if (!build_block_items(tbl, nedge, na, xtiles, ytiles, items)) return 13;
+          if (items.size() > 32767) return 10;   // TileSeq.nitems is 16-bit
+          ts.blocks += 1;
+          ts.sub_blocks += first_sub ? 0 : 1;
+          for (int g2 = 0; g2 < na * 4; ++g2) {
+            const int pb = tbl[4 * g2], mb = tbl[4 * g2 + 1], se = tbl[4 * g2 + 2], pe2 = tbl[4 * g2 + 3];
+            const int ps = pe2 > se ? ((se + 3) & ~3) : se;
+            ts.max_edge_group = std::max(ts.max_edge_group, nedge[g2]);
+            ts.split_groups += mb - pb > kChunkBeams ? 1 : 0;
+            ts.multi_entries += (se - mb) / 2 + (pe2 - ps) / 2;   // weighted entries: singles + both entries of every pair
+            for (int k = mb; k < se; k += 2) ts.max_multiplicity = std::max(ts.max_multiplicity, (int32_t)pay[k + 1]);
+            for (int k = ps; k < pe2; k += 4) ts.max_multiplicity = std::max(ts.max_multiplicity, (int32_t)pay[k + 2]);
+            ts.max_plain_group = std::max(ts.max_plain_group, mb - pb);
+          }
+          const size_t hdr = ((items.size() * 8) + 15) & ~(size_t)15;
+          const size_t bytes = std::max<size_t>(16, (hdr + pay.size() * 2 + 15) & ~(size_t)15);
+          if (blob.size() + bytes > 0x7FFFFFF0u) return 12;   // TileSeq.off is a 32-bit byte offset
+          TileSeq e{};
+          e.off = (int32_t)blob.size();
+          e.bytes = (int32_t)bytes;
+          e.chunk = (int16_t)v; e.stage = (int16_t)sg; e.a0 = (int16_t)a; e.nitems = (int16_t)items.size();
+          e.flags = (first_sub ? kSeqNewStage : 0u) | ((first_sub && si == 0) ? kSeqNewChunk : 0u) |
+                    ((first_sub && si == 0 && keep) ? kSeqKeepGrid : 0u);
+          if (first_sub)
+            for (int aa = ca0; aa < ca0 + cna; ++aa)
+              if (!cls[aa].wrap2[sg].empty()) e.flags |= kSeqHasWrap;
+          blob.resize(blob.size() + bytes, 0);
+          if (!items.empty()) std::memcpy(blob.data() + e.off, items.data(), items.size() * 8);
+          if (!pay.empty()) std::memcpy(blob.data() + e.off + hdr, pay.data(), pay.size() * 2);
+          seq.push_back(e);
+          a += na;
+          first_sub = false;
+        } while (a < ca0 + cna);
+      }
+      seq.back().flags |= kSeqEndChunk;
     }
   }
-  seq_start[(size_t)nq * C] = (int32_t)seq.size();
-  S.tile_stats[7] = (int32_t)lists.wrap2.size();
+  return 0;
+}
+
+// The kernel of plan p with its dynamic shared memory raised to the plan's, and its launch on ctas CTAs in clusters of p.C on
+// stream st (cfg, whose cluster attribute is at)
+static const void * tile_launch_config(const TilePlan & p, int ctas, cudaStream_t st, cudaLaunchConfig_t & cfg, cudaLaunchAttribute & at)
+{
+  const void * kfn = tile_kernel_for(p.pitch_w, p.tail != 0);
+  B200_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+  cfg = cudaLaunchConfig_t{};
+  cfg.gridDim = dim3((unsigned)ctas);
+  cfg.blockDim = dim3(kTileThreads);
+  cfg.dynamicSmemBytes = p.smem;
+  cfg.stream = st;
+  at.id = cudaLaunchAttributeClusterDimension;
+  at.val.clusterDim.x = (unsigned)p.C; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+  cfg.attrs = &at; cfg.numAttrs = 1;
+  return kfn;
+}
+
+bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st)
+{
+  const GridGeom & g = h->g;
+  const CorrPlan & p0 = S.plans[0];
+  const int nA = p0.nA, nq = S.nq;
+  auto bail = [&](int why) { S.tile_refusal = why; return false; };
+  if (const int why = parity_refusal(g, S.plans)) return bail(why);
+  // B200_TILE_TAIL=0 / B200_TILE_PAIRS=0 switch the tail layout / the weight-2 entries and pairing off, to measure each part alone
+  const TilePlan p = plan_tile({g.stride, g.height, p0.nX, p0.nY, nA, p0.n, S.max_n, S.do_penalize ? 1 : 0, S.npairs, h->sms,
+                                h->tile_cluster > 0 ? h->tile_cluster : env_int("B200_SWEEP_CLUSTER", 0),
+                                h->tile_chunks > 0 ? h->tile_chunks : env_int("B200_SWEEP_CHUNKS", 0),
+                                env_int("B200_TILE_TAIL", 1) != 0 ? 1 : 0});
+  if (p.refused) return bail(p.refused);
+  const bool pairs_on = env_int("B200_TILE_PAIRS", 1) != 0;
+
+  // ---- per-query descriptor blocks and schedules ----
+  const int nstage = 4 * p.nbands;
+  std::vector<uint8_t> blob;
+  std::vector<TileSeq> seq;
+  std::vector<int32_t> seq_start;
+  TileStats ts;
+  BeamLists lists;
+  std::vector<BeamClasses> cls(nA);
+  std::vector<Encoded> enc((size_t)nA * nstage);
+  blob.reserve((size_t)nq * nA * p0.n * 2 + 4096);
+  for (int q = 0; q < nq; ++q) {
+    host_parallel_for(nA, [&](int a) { encode_angle(g, S.plans[q], a, p, pairs_on, h->no_dedup, cls[a], &enc[(size_t)a * nstage]); });
+    append_beam_lists(cls, nstage, lists);
+    if (const int why = schedule_query(p, nA, cls, enc, blob, seq, seq_start, ts)) return bail(why);
+  }
+  seq_start.push_back((int32_t)seq.size());
+  ts.wrap2_entries = (int32_t)lists.wrap2.size();
   blob.resize(blob.size() + 16, 0);
 
   S.h2d(S.d_tile_desc, blob.data(), blob.size(), st);
   S.h2d(S.d_tile_seq, seq.data(), seq.size(), st);
   S.h2d(S.d_tile_seq_start, seq_start.data(), seq_start.size(), st);
   upload_beam_lists(lists, S, st);
+  TileDev & T = S.tile;
+  T = TileDev{};
+  T.C = p.C; T.V = p.V; T.nAc = p.nAc; T.nbands = p.nbands; T.band_rows = p.band_rows; T.alloc_rows = p.alloc_rows;
+  T.pitch_w = p.pitch_w; T.xtiles = p.xtiles; T.ytiles = p.ytiles; T.tail = p.tail; T.stage_bytes = p.stage_bytes;
+  T.int_ties = p.int_ties; T.off_A = p.off_A; T.off_probs = p.off_probs; T.off_stage = p.off_stage; T.off_cells = p.off_cells;
+  T.cell_cap = p.cell_cap;
+  raster_levels(g.kernel, g.ksize, T);
   T.desc = S.d_tile_desc.p; T.seq = S.d_tile_seq.p; T.seq_start = S.d_tile_seq_start.p;
   T.edge = S.d_edge.p; T.edge_start = S.d_edge_start.p;
   T.wrap2 = S.d_wrap2.p; T.wrap2_start = S.d_wrap2_start.p;
   T.slow = S.d_slow.p; T.slow_start = S.d_slow_start.p;
   T.enabled = 1;
-  S.tile_smem = smem;
 
   // ---- grid: as many co-resident clusters as the device holds, one pair per cluster at a time ----
-  const void * kfn = tile_kernel_for(pitch_w, T.tail != 0);
-  B200_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int max_clusters = sms / C;
-  {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(C * std::max(1, sms / C)));
-    cfg.blockDim = dim3(kTileThreads);
-    cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = (unsigned)C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    int nc = 0;
-    if (cudaOccupancyMaxActiveClusters(&nc, kfn, &cfg) == cudaSuccess && nc > 0) max_clusters = nc;
-    else (void)cudaGetLastError();
-  }
-  const int clusters = std::max(1, std::min(S.npairs, max_clusters));
-  S.tile_grid = clusters * C;
-  S.tile_info[0] = 1; S.tile_info[1] = C; S.tile_info[2] = V; S.tile_info[3] = nbands; S.tile_info[4] = B; S.tile_info[5] = 0;
-  S.tile_info[6] = clusters; S.tile_info[7] = (int32_t)(smem / 1024);
-  S.tile_layout[0] = ytile_rows; S.tile_layout[1] = ytiles; S.tile_layout[2] = xtiles; S.tile_layout[3] = tail ? 1 : 0;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at;
+  const void * kfn = tile_launch_config(p, p.C * std::max(1, h->sms / p.C), nullptr, cfg, at);
+  int max_clusters = h->sms / p.C, nc = 0;
+  if (cudaOccupancyMaxActiveClusters(&nc, kfn, &cfg) == cudaSuccess && nc > 0) max_clusters = nc;
+  else (void)cudaGetLastError();
+  S.tile_plan = p;
+  S.tile_clusters = std::max(1, std::min(S.npairs, max_clusters));
+  S.tile_stats = ts;
+  S.tile_refusal = 0;
   return true;
 }
 
 void launch_sweep_tile(SweepHost & S, cudaStream_t st)
 {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)S.tile_grid);
-  cfg.blockDim = dim3(kTileThreads);
-  cfg.dynamicSmemBytes = S.tile_smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = (unsigned)S.tile.C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  const void * kfn = tile_kernel_for(S.tile.pitch_w, S.tile.tail != 0);
-  B200_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S.tile_smem));
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at;
+  const void * kfn = tile_launch_config(S.tile_plan, S.tile_clusters * S.tile_plan.C, st, cfg, at);
   void * args[] = {(void *)&S.dev, (void *)&S.tile};
   B200_CUDA(cudaLaunchKernelExC(&cfg, kfn, args));
 }

@@ -201,6 +201,29 @@ struct TileDev {
   const int32_t * slow_start;    // [nq][nA + 1]
 };
 
+// What the tiled kernel's planner (plan_tile) decides from: the grid (row stride, height), the coarse pose window, the beams of a
+// query, the longest candidate scan rounded up to 4 readings (SweepHost::max_n), the batch and the device's SMs; cluster / chunks
+// force the cluster size / a minimum number of angle chunks (0 = automatic), tail = 0 keeps 48-row y-tiles everywhere.
+struct TilePlanIn {
+  int stride, height, nX, nY, nA, n, max_n, do_penalize, npairs, sms, cluster, chunks, tail;
+};
+// The planner's result: a refusal code (2, 4, 5, 9: see plan_tile) or the chunking, banding and shared-memory layout the kernel
+// runs with (the fields of TileDev of the same names).
+struct TilePlan {
+  int refused = 0;
+  int C = 0, V = 0, nAc = 0, nbands = 0, band_rows = 0, alloc_rows = 0, pitch_w = 0;
+  int xtiles = 0, ytiles = 0, ytile_rows = 0, tail = 0, stage_bytes = 0, int_ties = 0;
+  size_t off_A = 0, off_probs = 0, off_stage = 0, off_cells = 0;
+  int cell_cap = 0;
+  size_t smem = 0;               // dynamic shared memory per CTA
+};
+TilePlan plan_tile(const TilePlanIn & in);
+// What the tiled kernel's descriptor blocks hold: the stats of b200sm_batch_tile_stats, in its order
+struct TileStats {
+  int32_t blocks = 0, sub_blocks = 0, max_edge_group = 0, split_groups = 0, multi_entries = 0, max_multiplicity = 0,
+          max_plain_group = 0, wrap2_entries = 0;
+};
+
 struct FineDev {
   int P, nA;
   const int32_t * offsets;   // [npairs][nA][n]
@@ -246,13 +269,12 @@ struct SweepHost {
   int fast_blocks = 0;
   int32_t fast_refusal = 0;   // why build_fast_tables last refused a sweep (0 = it built its tables)
   TileDev tile{};
-  size_t tile_smem = 0;
-  int tile_grid = 0;
-  int32_t tile_info[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // enabled, C, V, nbands, band rows, refusal reason, clusters, smem KB
-  // what the tiled kernel's descriptor blocks contain (b200sm_batch_tile_stats): blocks, continuation sub-blocks, largest EDGE
-  // group, groups cut into pieces, multi entries, largest multiplicity, largest plain group, wrap2 entries
-  int32_t tile_stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  int32_t tile_layout[4] = {0, 0, 0, 0};   // rows per y-tile (40 or 48), y-tiles, x-tiles, tail row (b200sm_batch_tile_layout)
+  // the plan, resident clusters (the grid is tile_clusters x tile_plan.C CTAs) and block contents of the tiled kernel when the
+  // upload runs it, zero otherwise (b200sm_batch_tile_info / _layout / _stats)
+  TilePlan tile_plan{};
+  int tile_clusters = 0;
+  TileStats tile_stats{};
+  int32_t tile_refusal = 0;   // why build_tile_tables last refused a sweep (0 = it built its tables)
   DevBuf<uint8_t> d_tile_desc;
   DevBuf<TileSeq> d_tile_seq;
   DevBuf<int32_t> d_tile_seq_start;
@@ -367,7 +389,7 @@ void encode_runs(const std::vector<uint16_t> & group, int min_weight, bool merge
 // steps of exactly 2 cells in x (6) and y (7) in every plan.
 int parity_refusal(const GridGeom & g, const std::vector<CorrPlan> & plans);
 
-// The builders of the parity kernels' tables return false, with a refusal code in fast_refusal / tile_info[5], when their kernel
+// The builders of the parity kernels' tables return false, with a refusal code in fast_refusal / tile_refusal, when their kernel
 // cannot run the uploaded sweep.  They copy nothing to the device before their last refusal.
 bool build_fast_tables(b200sm * h, SweepHost & S, cudaStream_t st);
 bool build_tile_tables(b200sm * h, SweepHost & S, cudaStream_t st);

@@ -1,5 +1,5 @@
-"""Plain-Python restatement of the tiled sweep kernel's planner (build_tile_tables in csrc/sm_tile.cu), written from the code,
-for tests that check which plan the device reports at geometries the shipped parameters never reach.
+"""Plain-Python restatement of the tiled sweep kernel's planner (plan_tile in csrc/sm_tile.cu), written from the code, for tests
+that check which plan the device reports at geometries the shipped parameters never reach.
 
 The planner takes the correlation grid (stride, height), the coarse pose window (nX x nY poses, nA angles), the query's beam
 count n, whether the sweep is penalised (the per-cell image is then FP64 instead of int32 sums), the batch size and the device's
