@@ -133,6 +133,8 @@ def lib():
         L.b200pg_default_opts.argtypes = [C.POINTER(PgOpts)]
         L.b200pg_create.argtypes = [C.POINTER(PgOpts), C.POINTER(C.c_void_p)]
         L.b200pg_destroy.argtypes = [C.c_void_p]
+        L.b200pg_set_opts.argtypes = [C.c_void_p, C.POINTER(PgOpts)]
+        L.b200pg_get_opts.argtypes = [C.c_void_p, C.POINTER(PgOpts)]
         L.b200pg_set_stream.argtypes = [C.c_void_p, C.c_void_p]
         L.b200pg_reset.argtypes = [C.c_void_p]
         L.b200pg_clear.argtypes = [C.c_void_p]
@@ -466,16 +468,36 @@ class ScanSolver:
     (solvers/ceres_solver.cpp), on the GPU."""
 
     def __init__(self, **opts):
+        o = self._options(opts)
+        self.opts = o
+        self._h = C.c_void_p()
+        _check(lib().b200pg_create(C.byref(o), C.byref(self._h)))
+        self.summary = None
+        self._node_ids = {}   # the ids in the node store, for getGraph (the C API reads poses by id)
+
+    @staticmethod
+    def _options(opts):
+        """The default options with `opts` set; an unknown key raises KeyError."""
         o = PgOpts()
         lib().b200pg_default_opts(C.byref(o))
         for k, v in opts.items():
             if not hasattr(o, k):
                 raise KeyError(k)
             setattr(o, k, v)
+        return o
+
+    def SetOptions(self, **opts):
+        """b200pg_set_opts (CeresSolver::Configure on a live solver): the default options with `opts` set, as the
+        constructor takes them; the graph and the corrections are kept.  Invalid options raise and change nothing."""
+        o = self._options(opts)
+        _check(lib().b200pg_set_opts(self._h, C.byref(o)))
         self.opts = o
-        self._h = C.c_void_p()
-        _check(lib().b200pg_create(C.byref(o), C.byref(self._h)))
-        self.summary = None
+
+    def GetOptions(self) -> PgOpts:
+        """b200pg_get_opts: the options the next Compute uses."""
+        o = PgOpts()
+        _check(lib().b200pg_get_opts(self._h, C.byref(o)))
+        return o
 
     def close(self):
         if self._h:
@@ -493,6 +515,7 @@ class ScanSolver:
 
     def Reset(self):
         _check(lib().b200pg_reset(self._h))
+        self._node_ids.clear()
 
     def Clear(self):
         _check(lib().b200pg_clear(self._h))
@@ -500,6 +523,7 @@ class ScanSolver:
     def AddNode(self, unique_id: int, corrected_pose):
         p = np.ascontiguousarray(corrected_pose, dtype=np.float64)
         _check(lib().b200pg_add_node(self._h, int(unique_id), _dp(p)))
+        self._node_ids.setdefault(int(unique_id))   # an id already stored keeps its entry, as in the store
 
     def AddConstraint(self, source_id: int, target_id: int, pose_difference, covariance) -> bool:
         """LinkInfo::GetPoseDifference() / GetCovariance(). Returns False where the reference warns and ignores."""
@@ -516,6 +540,7 @@ class ScanSolver:
         if rc == ERR_NOT_FOUND:
             return False
         _check(rc)
+        del self._node_ids[int(unique_id)]
         return True
 
     def RemoveConstraint(self, source_id: int, target_id: int) -> bool:
@@ -537,8 +562,9 @@ class ScanSolver:
         return None if rc == ERR_NOT_FOUND else p[2]
 
     def getGraph(self):
-        n = lib().b200pg_num_nodes(self._h)
-        return {i: self.get_node(i) for i in self._ids()} if n else {}
+        """ScanSolver::getGraph: {id: pose} of every node in the store."""
+        assert len(self._node_ids) == lib().b200pg_num_nodes(self._h)
+        return {i: self.get_node(i) for i in self._node_ids}
 
     def get_node(self, unique_id: int):
         p = np.zeros(3)

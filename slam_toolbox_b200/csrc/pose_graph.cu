@@ -802,8 +802,8 @@ static void minimize(Launcher & L, Strategy & strategy, b200pg_summary & S)
     const double * sc = h->h_scalars.p;
     strategy.fetched(sc, it, S);
     const double model_cost_change = sc[4], step_norm = sqrt(sc[5]), cand_cost = sc[1];
-    const bool finite = std::isfinite(model_cost_change) && std::isfinite(cand_cost) && std::isfinite(sc[9]);
-    if (!finite || !(model_cost_change > 0.0)) {
+    // only a failed linear solve or a model cost change that is not positive makes the step invalid
+    if (!std::isfinite(model_cost_change) || !std::isfinite(sc[9]) || !(model_cost_change > 0.0)) {
       if (invalid_step()) break;
       continue;
     }
@@ -814,7 +814,9 @@ static void minimize(Launcher & L, Strategy & strategy, b200pg_summary & S)
     const double rel = (ev_cur - cand_cost) / model_cost_change;
     const double hist = (ev_ref - cand_cost) / (acc_ref + model_cost_change);
     const double quality = std::max(rel, hist);
-    if (!(quality > o.min_relative_decrease)) {
+    // a candidate whose cost is not finite is a valid step of the lowest quality (TrustRegionStepEvaluator::StepQuality):
+    // rejected, not invalid
+    if (!std::isfinite(cand_cost) || !(quality > o.min_relative_decrease)) {
       strategy.rejected();
       continue;
     }
